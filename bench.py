@@ -2,6 +2,7 @@
 """bench.py -- headline benchmark of the MSM / NTT hot paths.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--lg-msm 26] [--lg-ntt 24]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one BLS12-381 G1 MSM over 2^26 synthetic points (BASELINE.json's headline metric),
@@ -11,7 +12,11 @@ through the drop-in C-ABI `mult_pippenger` with HOST (pinned) buffers (at N > 1:
 shard through `mult_pippenger`, then the same all-gather + combine).  The Goldilocks 2^24 NTT
 (the metric's second half) is measured in the same run and reported under "ntt".
 Timing: CUDA events on the launching stream, barrier + synchronize on both sides, max over
-ranks.  Inputs (8.6 GB MSM, 2 x 128 MiB NTT + L2 flush) exceed the 126 MB L2.
+ranks.  Inputs (8.6 GB MSM, 2 x 128 MiB NTT + L2 flush) exceed the 50 MB L2 of an H100.
+
+--dump-outputs DIR writes, after the timed steps, what the timed legs computed in their last
+step as DIR/<name>.npy (float64, at most 64 MB in all); the inputs are seeded, so two builds run
+with the same arguments can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -39,7 +44,7 @@ def measured_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 class ClockSampler:
@@ -120,6 +125,41 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm), "source": "nvidia-smi -lms 200"}
 
 
+P_BLS = 0x1a0111ea397fe69a4b1ba7b6434bacd764774b84f38512bf6730d2a0f6b0f6241eabfffeb153ffffb9feffffffffaaab
+P_PALLAS = 0x40000000000000000000000000000000224698fc094cf91b992d30ed00000001
+DUMP_NTT_SAMPLE = 1 << 20       # NTT elements kept by --dump-outputs (a fixed, seeded sample)
+
+
+def affine_words(jac, p, nl):
+    """A Jacobian result (3 x nl Montgomery limbs) as its affine normal form (x, y), each as
+    2*nl little-endian 32-bit words in float64 (exact).  The Jacobian triple of a group element
+    is not unique, the affine point is; the point at infinity is all zeros."""
+    limbs = np.asarray(jac, dtype=np.uint64)
+    to_int = lambda k: sum(int(v) << (64 * i) for i, v in enumerate(limbs[k * nl:(k + 1) * nl]))   # noqa: E731
+    rinv = pow(1 << (64 * nl), -1, p)
+    X, Y, Z = (to_int(k) * rinv % p for k in range(3))
+    out = np.zeros((2, 2 * nl), dtype=np.float64)
+    if Z:
+        zi = pow(Z, -1, p)
+        for row, v in enumerate((X * zi * zi % p, Y * zi * zi * zi % p)):
+            out[row] = [(v >> (32 * i)) & 0xFFFFFFFF for i in range(2 * nl)]
+    return out
+
+
+def u64_words(a):
+    """uint64 array -> (n, 2) float64 of its low and high 32-bit words (exact)"""
+    a = np.asarray(a, dtype=np.uint64)
+    return np.stack([(a & np.uint64(0xFFFFFFFF)).astype(np.float64), (a >> np.uint64(32)).astype(np.float64)], axis=-1)
+
+
+def dump_outputs(outdir, arrays):
+    os.makedirs(outdir, exist_ok=True)
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= 64 << 20, f"--dump-outputs: {total} bytes exceed 64 MB"
+    for name, a in arrays.items():
+        np.save(os.path.join(outdir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float64))
+
+
 def fold_scalars(sc, m, r=None):
     """sum of scalars per residue class i mod m, reduced mod r -> (m, 4) uint64."""
     r = R_BLS if r is None else r
@@ -140,7 +180,7 @@ def fold_scalars(sc, m, r=None):
 
 def cpu_reference_msm(points, scalars, nthreads):
     """sppark's CPU path on the host cores: the reference's own msm/pippenger.hpp when oracle/_ref
-    holds it (built in the authoring container from /root/reference), else the C restatement."""
+    holds it (built from a reference checkout, oracle/Makefile), else the C restatement."""
     from oracle import pyoracle
     t0 = time.perf_counter()
     if pyoracle.ref_cpu() is not None:
@@ -216,7 +256,11 @@ def main():
     ap.add_argument("--skip-cpu", action="store_true")
     ap.add_argument("--skip-ref-gpu", action="store_true")
     ap.add_argument("--lg-pallas", type=int, default=24)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float64)")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -297,6 +341,7 @@ def main():
     barrier()
     clocks = sampler.stop()
     gpu_launches = _lib.launch_count() - launches1
+    outputs = {"msm_bls12_381_g1_affine": affine_words(np.asarray(result, dtype=np.uint64), P_BLS, 6)}
     ms_step = max_over_ranks(e0.elapsed_time(e1) / args.steps)
     value = 1e3 / ms_step
 
@@ -313,21 +358,13 @@ def main():
     alg_bytes = n * 128                              # 96-B affine point + 32-B scalar, read once
     acc = sum(acc_ms) / len(acc_ms)
     achieved = alg_bytes / (acc * 1e-3) / 1e9 if acc > 0 else 0.0
-    # DRAM traffic of this kernel at 2^26 / c=20 from the committed `ncu --set full` capture
-    # (profiles/msm_accumulate_r01.md: dram__bytes_read.sum + dram__bytes_write.sum per launch);
-    # every point is gathered once per window, hence ~19x the algorithmic bytes
-    traffic = 174.7e9 if (args.lg_msm == 26 and world == 1) else None      # profiles/msm_accumulate_r01.md (kernel unchanged)
-    wide_mults = 2880.0 * phases_entries(n, world)          # 10 products x 288 IMAD.WIDE per mixed add
-    imad_peak = 0.94 * 32 * 148 * 1.965e9                   # measured: tools/imad_bench.cu on this B200
+    # the kernel's DRAM traffic is not measured (every point is gathered once per window, so it
+    # is a multiple of the algorithmic bytes); the fraction below is of algorithmic bytes
     roofline = {"bound": "hbm", "kernel": "msm::accumulate_kernel", "achieved": achieved, "peak": peak,
-                "unit": "GB/s", "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
+                "unit": "GB/s", "frac": achieved / peak, "traffic": None, "peak_source": peak_src,
                 "kernel_ms": acc, "phases_ms": phases,
-                "int32_issue": {"achieved_wide_mults_per_s": wide_mults / (acc * 1e-3) if acc > 0 else 0.0,
-                                "peak_wide_mults_per_s": imad_peak,
-                                "frac": (wide_mults / (acc * 1e-3) / imad_peak) if acc > 0 else 0.0,
-                                "note": "IMAD.WIDE.U32 issues at 0.94 warp-instr/clk/SM (tools/imad_bench.cu)"},
-                "note": "bucket accumulation is bounded by INT32 multiply issue, not HBM; the HBM fraction is "
-                        "reported because the contract asks for it (DESIGN.md section 5)"}
+                "note": "bucket accumulation is integer-multiply work (Montgomery products), so the HBM "
+                        "fraction of its algorithmic bytes is low by construction (DESIGN.md section 5)"}
 
     # ---- self-check at full size (size-independent property, no oracle): folding the scalars of
     # the replicated points onto the m distinct points must give the same group element
@@ -405,12 +442,12 @@ def main():
                "note": "--skip-e2e"}
 
     # ---------------------------------------------------------------- Goldilocks NTT (second half of the metric)
-    ntt_res = bench_ntt(args, torch, ntt, _lib, peak, peak_src, barrier, max_over_ranks, world)
+    ntt_res = bench_ntt(args, torch, ntt, _lib, peak, peak_src, barrier, max_over_ranks, world, outputs)
 
     # ---------------------------------------------------------------- config 4: Pallas MSM, sharded like the headline
-    pallas = bench_pallas(args, torch, msm, parallel, barrier, max_over_ranks, rank, world)
+    pallas = bench_pallas(args, torch, msm, parallel, barrier, max_over_ranks, rank, world, outputs)
 
-    # ---------------------------------------------------------------- the reference's own sm_100a kernels (N = 1)
+    # ---------------------------------------------------------------- the reference's own kernels, sm_90a (N = 1)
     ref_gpu = None
     if world == 1 and need_host and not args.skip_ref_gpu:
         ref_gpu = bench_reference_gpu(args, torch, msm, ntt, _lib, pts_host, sc_host, e2e_result, e2e)
@@ -440,19 +477,10 @@ def main():
                 "cpu_baseline": cpu, "check": check, "ntt": ntt_res, "pallas_msm": pallas,
                 "reference_gpu": ref_gpu}
         emit(line)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, outputs)
     if world > 1:
         dist.destroy_process_group()
-
-
-def phases_entries(n, world):
-    """mixed additions of one accumulate launch: one per (point, window), c chosen as the library does."""
-    best = None
-    for c in range(4, 23):
-        w = (256 + c - 1) // c
-        cost = w * (1.11 * n + 5.5 * (1 << (c - 1)))
-        if best is None or cost < best[0]:
-            best = (cost, w)
-    return best[1] * n
 
 
 def _jac_equal(a, b, msm, field=0, nl=6):
@@ -475,7 +503,7 @@ def _jac_equal(a, b, msm, field=0, nl=6):
 R_PALLAS = 0x40000000000000000000000000000000224698fc0994a8dd8c46eb2100000001   # order of the Pallas group
 
 
-def bench_pallas(args, torch, msm, parallel, barrier, max_over_ranks, rank, world):
+def bench_pallas(args, torch, msm, parallel, barrier, max_over_ranks, rank, world, outputs):
     """BASELINE.json config 4: Pallas MSM over 2^24 points, sharded by point-chunk over the ranks
     (2^21 points per GPU at N = 8), one all-gather of the 96-byte partial results + combine.
     Device-resident, strong scaling; checked by folding every rank's scalars onto the distinct
@@ -506,6 +534,7 @@ def bench_pallas(args, torch, msm, parallel, barrier, max_over_ranks, rank, worl
         e1.record()
         barrier()
         ms = max_over_ranks(e0.elapsed_time(e1) / iters)
+        outputs["msm_pallas_affine"] = affine_words(np.asarray(result, dtype=np.uint64), P_PALLAS, 4)
         folded = fold_scalars(sc, m, R_PALLAS)
         if world > 1:
             parts = parallel.all_gather_partials(folded.reshape(-1), "cuda").reshape(world * m, 4)
@@ -528,10 +557,10 @@ class _RustError(C.Structure):
 
 def bench_reference_gpu(args, torch, msm, ntt, _lib, pts_host, sc_host, ours_result, ours_e2e):
     """The kernels to beat: the REFERENCE's own CUDA code (poc/msm-cuda/cuda/pippenger.cu and
-    poc/ntt-cuda/cuda/ntt_api.cu) compiled for sm_100a into oracle/_ref by oracle/Makefile, called
+    poc/ntt-cuda/cuda/ntt_api.cu) compiled for sm_90a into oracle/_ref by oracle/Makefile, called
     through the identical host-pointer entry points on the same buffers, pinned and pageable, and
     (NTT) on device-resident data.  Runs after the repository's own timed regions; rank 0, N = 1."""
-    out = {"source": "oracle/_ref/*.so = the reference's sources built with nvcc -arch sm_100a (oracle/Makefile)"}
+    out = {"source": "oracle/_ref/*.so = the reference's sources built with nvcc for sm_90a (oracle/Makefile)"}
     refdir = os.path.join(ROOT, "oracle", "_ref")
     n = pts_host.shape[0]
     try:
@@ -651,7 +680,7 @@ def bench_reference_gpu(args, torch, msm, ntt, _lib, pts_host, sc_host, ours_res
 
 def bench_polynomial(args, torch, _lib, refdir):
     """SURVEY.md section 8 row f4 next to the reference's own polynomial/ kernels (oracle/ref_poly.cu
-    built for sm_100a): Goldilocks, 2^lg_ntt elements resident in HBM (128 MiB at 2^24, larger
+    built for sm_90a): Goldilocks, 2^lg_ntt elements resident in HBM (128 MiB at 2^24, larger
     than L2), CUDA events on the stream each side launches on, mean of 10 calls back to back."""
     path = os.path.join(refdir, "libref_poly_gl64_gpu.so")
     if not os.path.exists(path):
@@ -708,7 +737,7 @@ def bench_polynomial(args, torch, _lib, refdir):
     return {"workload": f"Goldilocks, 2^{args.lg_ntt} elements, device resident", **rows}
 
 
-def bench_ntt(args, torch, ntt, _lib, peak, peak_src, barrier, max_over_ranks, world):
+def bench_ntt(args, torch, ntt, _lib, peak, peak_src, barrier, max_over_ranks, world, outputs):
     """Goldilocks 2^lg NTT, NN order, device-resident (NTT::Base_dev_ptr path) and e2e
     (compute_ntt with a pinned host buffer).  With N > 1 ranks ONE transform is slab-sharded over
     the ranks (column slabs, one NCCL all-to-all between the two local passes; strong scaling)."""
@@ -736,6 +765,12 @@ def bench_ntt(args, torch, ntt, _lib, peak, peak_src, barrier, max_over_ranks, w
         e1.synchronize()
         tot += e0.elapsed_time(e1)
     ms = max_over_ranks(tot / iters)
+    out = d.cpu().numpy().view(np.uint64)
+    if n > DUMP_NTT_SAMPLE:
+        idx = np.sort(np.random.default_rng(0).choice(n, size=DUMP_NTT_SAMPLE, replace=False))
+        outputs["ntt_gl64_sample_index"] = idx.astype(np.float64)
+        out = out[idx]
+    outputs["ntt_gl64_words"] = u64_words(out)
     _lib.profile_enable(True)
     flush.zero_()
     ntt.ntt_dev(d, ntt.NN)
@@ -749,16 +784,7 @@ def bench_ntt(args, torch, ntt, _lib, peak, peak_src, barrier, max_over_ranks, w
            "roofline": {"bound": "hbm", "kernel": "ntt::pass_kernel_static<gl64, 12 x 2> (slowest of the two block-tile passes)",
                         "achieved": alg / (worst * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
                         "frac": alg / (worst * 1e-3) / 1e9 / peak,
-                        # dram__bytes_read.sum + dram__bytes_write.sum of that pass from the ncu --set full
-                        # capture (profiles/ntt_block_r02.md, launch 0: 134.4 MB + 87.6 MB), 2^24 only
-                        "traffic": 222.1e6 if lg == 24 else None, "traffic_source": "profiles/ntt_block_r02.md",
-                        "peak_source": peak_src,
-                        # the binding resource is the INT32 ALU pipe, not HBM: the butterfly network alone
-                        # (tools/gl64_bfly_bench.cu, profiles/gl64_butterfly_microbench_r02.txt) needs 37.9
-                        # SMSP-cycles per butterfly at 90 % ALU-pipe utilisation
-                        "int32_alu": {"butterflies": n // 2 * lg, "dense_cycles_per_butterfly": 37.9,
-                                      "floor_ms": (n // 2 * lg / 32) * 37.9 / (148 * 4) / 1.965e6,
-                                      "frac": ((n // 2 * lg / 32) * 37.9 / (148 * 4) / 1.965e6) / ms},
+                        "traffic": None, "peak_source": peak_src,
                         "pass_ms": [round(p, 4) for p in passes],
                         "whole_transform_frac": alg / (ms * 1e-3) / 1e9 / peak}}
     # e2e: in place on the pinned host buffer through compute_ntt

@@ -1,5 +1,5 @@
 /*
- * sppark_b200.h -- C ABI of libsppark_b200.so, the B200-native MSM / NTT library.
+ * sppark_b200.h -- C ABI of libsppark_b200.so, the H100-native (sm_90a) MSM / NTT library.
  *
  * The first block is the DROP-IN surface: the exact symbols, signatures and error
  * convention that supranational/sppark's PoC crates bind through FFI, so that a caller of

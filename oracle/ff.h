@@ -4,7 +4,7 @@
  * Portable Montgomery prime-field arithmetic on 64-bit limbs (unsigned
  * __int128 products).  It stands in for the host-side field types the
  * reference takes from third-party code that is NOT vendored under
- * /root/reference:
+ * the reference tree:
  *   - blst  src/blst_t.hpp  (crate blst ~0.3.11, poc/msm-cuda/Cargo.toml:24)
  *       -> blst_384_t / blst_256_t, used by ff/bls12-381.hpp:91-139
  *   - semolina pasta_t.hpp  (crate semolina ~0.1.2, poc/ntt-cuda/Cargo.toml:28)

@@ -11,7 +11,7 @@ poc/msm-cuda/cuda/pippenger_inf.cu:8-13,36-47), restated on Python integers:
 The C oracle (oracle/ec2.c) covers BLS12-381 G2 only; these two curves are small additions on top of
 the same kernels, so a slow, obviously-right restatement is enough.  Pinned by
 tests/golden/msm_g2_curves2_ref_gpu.npz: outputs of the reference's own CUDA templates for these
-features (oracle/ref_msm_g2.cu built with FEATURE_BN254 / FEATURE_BLS12_377, run on a B200 by
+features (oracle/ref_msm_g2.cu built with FEATURE_BN254 / FEATURE_BLS12_377, run on a GPU by
 tests/golden/make_golden.py g2_curves2).
 
 Memory formats (what the C ABI carries): Fp = `nl` 64-bit little-endian limbs, Montgomery form

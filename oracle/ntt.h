@@ -16,7 +16,7 @@
  *            transform as NN (ntt/ntt.cuh:186-189,211-212; poc/ntt-cuda/tests/ntt.rs:28-30
  *            asserts NN == RR), with bit-reversed coset exponents.  ORACLE_BB (4) is the strict
  *            bit-reversed-in / bit-reversed-out transform (an extension, not a reference order).
- *            Pinned by tests/golden/ntt_ref_gpu.npz (the reference's own kernels on a B200).
+ *            Pinned by tests/golden/ntt_ref_gpu.npz (the reference's own CUDA kernels).
  * Root conventions (derived, and checked against the ntt/parameters headers by
  * tests/test_params_pin.py):
  *   Goldilocks  w_2^32 = 7^((p-1)/2^32), group_gen = 7   (goldilocks.h:84-160, default branch)

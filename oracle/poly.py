@@ -13,7 +13,7 @@ inversion compute (the reference code is cooperative CUDA; the arithmetic it per
   batch_inversion      ff/batch_inversion.hpp:14-51: out[i] = 1 / inp[i], zero where inp[i] == 0
 
 Pinned by tests/golden/poly_ref_gpu.npz: outputs of the reference's own kernels (oracle/ref_poly.cu
-compiled from /root/reference, run on a B200 by tests/golden/make_golden.py gen_poly); the
+compiled from the reference sources, run on a GPU by tests/golden/make_golden.py gen_poly); the
 reference itself holds no test or vector for these templates.  batch_inversion is header-only with
 no entry point in the reference; it is pinned by its defining property (x * x^-1 == 1) only.
 

@@ -2,7 +2,7 @@
 
 liboracle.so   = the C restatement (oracle/ff.c ec.c ec2.c msm.c ntt.c)
 _ref/*.so      = the reference's own sources compiled where they lie (oracle/Makefile),
-                 present only if built in the authoring container.
+                 present only where a reference checkout was given (SPPARK_REFERENCE).
 All buffers are numpy arrays; field elements are little-endian 64-bit limbs.
 """
 import ctypes as C
@@ -33,9 +33,11 @@ def build(force=False):
 
 
 def build_ref():
-    """Compile the reference's own sources into oracle/_ref (authoring container only)."""
-    if os.path.isdir("/root/reference"):
-        subprocess.check_call(["make", "-s", "-C", HERE, "ref"])
+    """Compile the reference's own sources into oracle/_ref, from the supranational/sppark checkout
+    named by $SPPARK_REFERENCE (nothing is built without one)."""
+    ref = os.environ.get("SPPARK_REFERENCE", "")
+    if ref and os.path.isdir(ref):
+        subprocess.check_call(["make", "-s", "-C", HERE, "ref", "REF=" + os.path.abspath(ref)])
         return True
     return False
 

@@ -2,7 +2,7 @@
  * oracle/ref_msm_cpu.cpp -- TEST INFRASTRUCTURE ONLY.
  *
  * Thin extern "C" door onto the REFERENCE's own CPU Pippenger, compiled from
- * the sources where they lie under /root/reference (msm/pippenger.hpp:218,
+ * the sources where they lie in the reference tree (msm/pippenger.hpp:218,
  * ec/*.hpp, util/thread_pool_t.hpp) with oracle/shim/blst_t.hpp supplying the
  * un-vendored blst host field.  Built into oracle/_ref/ by oracle/Makefile;
  * used to validate the C restatement (oracle/msm.c) and as the "reference"

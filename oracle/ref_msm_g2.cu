@@ -9,7 +9,7 @@
  * built as _ref/libref_msm_g2_gpu.so)?  Its Affine_inf_t<fp2_t>::mem_t (ec/affine_t.hpp:95-97) is
  * sized from sizeof(field_t), which is 96 bytes in nvcc's host pass (host fp2_t = vec384x) but 48
  * in the device pass (device fp2_t = one fp_mont per lane): the host copies points with a
- * 224-byte pitch, the kernels index them with 208.  Recorded on a B200 (tests/golden/
+ * 224-byte pitch, the kernels index them with 208.  Recorded on a GPU (tests/golden/
  * make_golden.py g2): n = 1 is right, n = 2 returns s0*P0, n >= 33 is not even on the curve.
  * The packed affine_t has no such field, so this instantiation is consistent and pins G2.
  */

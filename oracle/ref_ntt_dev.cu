@@ -2,7 +2,7 @@
  * oracle/ref_ntt_dev.cu -- TEST INFRASTRUCTURE ONLY.
  * Device-pointer door onto the REFERENCE's own NTT (ntt/ntt.cuh:344-350 Base_dev_ptr),
  * compiled from the reference sources where they lie.  Lets bench/probe scripts time the
- * reference's kernels on the same B200 with data already resident ("the bar to beat").
+ * reference's kernels on the same GPU with data already resident ("the bar to beat").
  */
 #if defined(FEATURE_GOLDILOCKS)
 # include <ff/goldilocks.hpp>

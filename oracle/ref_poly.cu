@@ -3,7 +3,7 @@
  * Host-pointer doors onto the REFERENCE's own polynomial helpers, compiled from the reference
  * sources where they lie (polynomial/prefix_op.cuh:322, polynomial/div_by_x_minus_z.cuh:445,
  * polynomial/evaluate.cuh:308).  The reference ships no test or golden vector for these
- * templates, so tests/golden/make_golden.py runs them on a B200 through this shim and commits
+ * templates, so tests/golden/make_golden.py runs them on a GPU through this shim and commits
  * the input/output pairs (tests/golden/poly_ref_gpu.npz) -- that is what pins oracle/poly.py.
  */
 #if defined(FEATURE_GOLDILOCKS)

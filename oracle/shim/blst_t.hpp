@@ -2,7 +2,7 @@
  * oracle/shim/blst_t.hpp -- TEST INFRASTRUCTURE ONLY.
  *
  * Stand-in for blst's src/blst_t.hpp (crate blst ~0.3.11, not vendored under
- * /root/reference).  It provides exactly the host-field interface the
+ * the reference tree).  It provides exactly the host-field interface the
  * reference's own headers consume (ff/bls12-381.hpp:91-139, ec/*.hpp,
  * msm/pippenger.hpp, msm/pippenger.cuh host side) so that those headers
  * compile UNMODIFIED from where they lie; see oracle/Makefile.

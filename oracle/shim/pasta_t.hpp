@@ -2,7 +2,7 @@
  * oracle/shim/pasta_t.hpp -- TEST INFRASTRUCTURE ONLY.
  *
  * Stand-in for semolina's pasta_t.hpp (crate semolina ~0.1.2, poc/ntt-cuda/Cargo.toml:28; not
- * vendored under /root/reference), which the reference's ff/pasta.hpp:82-84 includes for its
+ * vendored in the reference tree), which the reference's ff/pasta.hpp:82-84 includes for its
  * HOST-side field types.  It provides the two class names that header expects, pallas_t and
  * vesta_t, on the same portable Montgomery class as oracle/shim/blst_t.hpp, so that
  * ff/pasta.hpp, ec/*.hpp and msm/pippenger.cuh compile UNMODIFIED from where they lie and the

@@ -1,5 +1,5 @@
 """ctypes loader of libsppark_b200.so.  There is no CPU fallback: if the CUDA library is
-missing or the machine has no B200-class device, calls fail loudly."""
+missing or the machine has no H100-class (sm_90) device, calls fail loudly."""
 import ctypes as C
 import os
 

@@ -1,7 +1,7 @@
-"""In-tree build of libsppark_b200.so (nvcc, sm_100a only).
+"""In-tree build of libsppark_b200.so (nvcc, sm_90a only).
 
-`python -m sppark_b200.build` or `__graft_entry__.build()`.  The .so is git-ignored but travels
-to the GPU box with the gpurun snapshot.
+`python -m sppark_b200.build` or `__graft_entry__.build()`.  The .so and the objects under
+build/ are build products (git-ignored).
 """
 import os
 import subprocess
@@ -14,9 +14,9 @@ LIB = os.environ.get("SPPARK_B200_LIB") or os.path.join(HERE, "libsppark_b200.so
 SOURCES = ["api.cu", "util/gpu.cu", "ntt/ntt.cu", "ntt/ntt_warp.cu", "poly/poly.cu", "msm/msm.cu", "msm/msm_bls12_381.cu", "msm/msm_bls12_381_g2.cu",
            "msm/msm_pasta.cu", "msm/msm_bn254_bls12_377.cu", "msm/msm_bn254_g2.cu", "msm/msm_bls12_377_g2.cu"]
 # the wide-product variants of the hot-loop multiplications (dedicated squaring, single-reduction
-# a*b - c*d, Karatsuba; ff/mont.cuh) measured SLOWER than the fused ladder on B200 (round 1:
-# accumulate 2^24: fused 111 ms, +msub 115, +sqr 126, +both 130), so they are compiled out
-NVCC_FLAGS = ["-std=c++17", "-O3", "-DSPPARK_B200_NO_WIDE_SQR", "-DSPPARK_B200_NO_WIDE_MSUB", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+# a*b - c*d, Karatsuba; ff/mont.cuh) are compiled out: the fused ladder is the default.  They have
+# not been measured on H100
+NVCC_FLAGS = ["-std=c++17", "-O3", "-DSPPARK_B200_NO_WIDE_SQR", "-DSPPARK_B200_NO_WIDE_MSUB", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "--threads", "4"]
 
 
@@ -68,7 +68,7 @@ def build(force=False, verbose=False):
     for p, cmd in procs:
         if p.wait() != 0:
             raise RuntimeError("nvcc failed: " + " ".join(cmd))
-    subprocess.check_call(["nvcc", "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a"])
+    subprocess.check_call(["nvcc", "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a"])
     return LIB
 
 

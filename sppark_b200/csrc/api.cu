@@ -21,7 +21,7 @@ extern "C" int sppark_b200_sm_count(int device_id)
     try { return select_gpu(device_id).sm_count(); } catch (...) { return -1; }
 }
 
-extern "C" const char* sppark_b200_version(void) { return "sppark_b200 0.1 (sm_100a)"; }
+extern "C" const char* sppark_b200_version(void) { return "sppark_b200 0.1 (sm_90a)"; }
 
 extern "C" uint64_t sppark_b200_launch_count(void) { return g_launch_count.load(); }
 

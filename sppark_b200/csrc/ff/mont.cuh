@@ -216,15 +216,15 @@ struct mont_t {
 
     // mul_shared / sqr_shared / msub_shared: ONE copy each per kernel, called (not inlined) from
     // the hot loop.  The unrolled ladder is ~450 instructions and a mixed add has ten products;
-    // inlining all of them overflows the instruction cache (ncu: no_instruction was the top
-    // stall before, 0.04 after; profiles/msm_accumulate_r01.md).  Only called from code that is
+    // inlining all of them overflows the instruction cache (no_instruction was the top stall
+    // reason before the split, measured on an earlier GPU).  Only called from code that is
     // itself inlined into the kernel, so the call depth is one.
 #if defined(__CUDA_ARCH__)
     // ---- double-width arithmetic for the hot loop -----------------------------------------
     // Products are kept unreduced (2N limbs) so that (a) a squaring can skip the mirrored half
     // of its partial products, (b) a*b - c*d needs ONE Montgomery reduction, (c) the a*b half
-    // can be split Karatsuba-style.  The IMAD.WIDE pipe is the bottleneck of the MSM (72 % busy,
-    // ALU pipe 27 %: profiles/msm_accumulate_r01.md), so trading wide multiplies for adds pays.
+    // can be split Karatsuba-style.  These trade wide multiplies (the IMAD.WIDE pipe is the busy
+    // one in the MSM) for adds; they are compiled out by default (sppark_b200/build.py).
     struct wide_t { uint32_t l[2 * N]; };
 
     // acc += x * v[0..W) at limb position I; even j into the file whose pairs sit at parity(I)
@@ -298,7 +298,7 @@ struct mont_t {
 #if defined(SPPARK_B200_KARATSUBA)
         constexpr bool karatsuba = N % 4 == 0 && N >= 8;
 #else
-        constexpr bool karatsuba = false;   // measured slower on B200: the extra live limbs spill (DESIGN.md section 5)
+        constexpr bool karatsuba = false;   // off: the extra live limbs spill (DESIGN.md section 5)
 #endif
         if constexpr (karatsuba) {
             constexpr int H = N / 2;

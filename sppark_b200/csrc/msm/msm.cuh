@@ -293,8 +293,7 @@ __global__ void finish_kernel(const Config cfg, const uint32_t* winR, uint32_t* 
 // ZZ*V, ZZZ*W}, a full addition four.  Lanes 0..3 of one warp execute the shared ladder in
 // lock-step on different operands (one instruction stream, SIMD), values travel through a few
 // shared-memory slots: 3 ladder latencies per doubling instead of 9, 4 per addition instead of
-// 14 (2.4 ms -> under 1 ms at 2^26; the same group element as finish_body, which the CPU
-// single-stepper keeps running).
+// 14 (the same group element as finish_body, which the CPU single-stepper keeps running).
 template<class F> struct Par4 {
     enum { sX, sY, sZZZ, sZZ, sA, sB, sC, sD, sE, sF, sG, sH, NS };
     // slot i of the accumulator: its four coordinates first, then eight scratch values that
@@ -574,10 +573,9 @@ public:
         COUNT_LAUNCH();
         // The scatter writes 4 random bytes per (point, window): with all windows in flight the
         // write set (4*n bytes per window) thrashes L2 and every store costs a 32-byte sector
-        // read + write-back in DRAM (ncu: 68 B of DRAM traffic per entry, profiles/msm_sort_r01.md).
-        // One launch per window confines the write set to one window's slots (4*n bytes, resident
-        // in the 126 MB L2 up to n = 2^24) at the price of re-reading the scalars per window:
-        // 11.4 -> 7.1 ms at 2^24, 44 -> 25 ms at 2^26.
+        // read + write-back in DRAM.  One launch per window confines the write set to one window's
+        // slots (4*n bytes, resident in the 50 MB L2 of an H100 up to n = 2^23) at the price of
+        // re-reading the scalars per window.
         bool per_window = n >= (1u << 18);
         if (const char* env = getenv("SPPARK_B200_MSM_SCATTER")) per_window = atoi(env) != 0;
         if (per_window) {

@@ -218,8 +218,8 @@ HD void accumulate_body(const Config& cfg, const uint32_t* points, const uint32_
         if (!live) return;
 #endif
         if (live) acc.madd(load_point<F>(points, DIRECT ? direct_base + k++ : run[k++]));
-        // (an explicit prefetch.global.L2 of the next point was measured: no gain at 2^24,
-        //  6 % slower at 2^26 -- the 12 resident warps per SM already cover the gather latency)
+        // (an explicit prefetch.global.L2 of the next point was tried: no gain on the GPU the
+        //  kernel was first tuned on -- the resident warps per SM already cover the gather latency)
     }
 }
 
@@ -280,7 +280,7 @@ HD void finish_body(const Config& cfg, const uint32_t* winR, uint32_t* out_jacob
     }
 }
 
-// window width minimising the measured cost model (B200, profiles/msm_phases_r01.txt):
+// window width minimising the measured cost model (fitted on an earlier GPU; not refitted for H100):
 //   per (point, window): 1 mixed add + ~0.11 for count/scatter;  per bucket: ~5.5 mixed-add
 //   equivalents for the two full adds of the running sum
 inline uint32_t choose_wbits(size_t npoints)
@@ -291,10 +291,10 @@ inline uint32_t choose_wbits(size_t npoints)
         uint32_t nwins = (256 + c - 1) / c;
         double cost = (double)nwins * (1.11 * (double)npoints + 5.5 * (double)(1u << (c - 1)));
         // a top window of only a few bits puts npoints / 2^e entries into each of its 2^e buckets: the
-        // count / scatter atomics collide on them and they go through the heavy-bucket path.  Measured
-        // at 2^23 points (the per-GPU share of the 8-GPU run): c = 18 (e = 4) 65.4 ms, c = 19 (e = 9)
-        // 64.6 ms against c = 16 (no thin window) 62.6 ms, where this model without the term ranks
-        // 18 first.  Left alone below 2^22 points, where the table was tuned without it.
+        // count / scatter atomics collide on them and they go through the heavy-bucket path; at 2^23
+        // points c = 16 (no thin window) measured faster than the c = 18 this model ranks first
+        // without the term (on the GPU the model was fitted on).  Left alone below 2^22 points,
+        // where the table was tuned without it.
         const uint32_t e = 256 - (nwins - 1) * c;                 // bits of the top window
         if (npoints >= ((size_t)1 << 22) && e <= 10 && (npoints >> e) > 2048) cost += 1.25 * (double)npoints;
         if (cost < best_cost) { best_cost = cost; best = c; }
@@ -314,7 +314,8 @@ inline Config make_config(size_t npoints)
     cfg.lg_nb = cfg.wbits - 1;
     cfg.npoints = (uint32_t)npoints;
     // a bucket is "heavy" when one lane folding it alone would take longer than that lane's fair
-    // share of the whole job (~57k lanes are resident on a B200): such buckets are cut into chunks
+    // share of the whole job (57k lanes: the resident lane count the constant was chosen for; an
+    // H100 keeps ~51k resident, close enough for a threshold): such buckets are cut into chunks
     // and spread over CTAs.  At 2^26 points the share is ~15k entries (nothing is heavy for uniform
     // scalars, the long top-window buckets are simply queued first); at 2^16 it is ~25, and the
     // three 16k-entry buckets of the top window must not be left to three single lanes.

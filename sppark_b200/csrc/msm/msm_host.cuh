@@ -85,14 +85,14 @@ RustError msm_host(void* out, const void* points, size_t npoints, const void* sc
             size_t k = std::max(1, atoi(env)), each = ((npoints + k - 1) / k + 31) & ~(size_t)31;
             for (size_t done = 0; done < npoints; done += each) sched.push_back(std::min(each, npoints - done));
         } else if (resident && npoints >= (1u << 22)) {
-            // only 32 B per point cross PCIe: N/8 then the rest (2^26: 394 ms; N/4 + 3N/4: 403;
-            // N/16 + 15N/16: 399; the four-slice schedule below: 408)
+            // only 32 B per point cross PCIe: N/8 then the rest (chosen over N/4 + 3N/4, N/16 +
+            // 15N/16 and the four-slice schedule below on an earlier GPU; not re-measured on H100)
             const size_t e = (npoints / 8 + 31) & ~(size_t)31;
             sched.push_back(e);
             sched.push_back(npoints - e);
         } else if (npoints >= (1u << 22)) {
-            // N/16, N/8, N/4, 9N/16 (measured at 2^26, tools/probe_e2e.py: 414 ms; N/8, N/8, N/4,
-            // N/2: 426 ms; five or six slices: 416-418 ms)
+            // N/16, N/8, N/4, 9N/16 (chosen over N/8, N/8, N/4, N/2 and five or six slices with
+            // tools/probe_e2e.py on an earlier GPU; not re-measured on H100)
             const size_t e = (npoints / 16 + 31) & ~(size_t)31;
             for (size_t part : {e, 2 * e, 4 * e}) sched.push_back(part);
             sched.push_back(npoints - 7 * e);

@@ -62,8 +62,8 @@ template<class F> bool launch_static(const Pass& d, const Tables<F>& tb, const t
                                      typename F::T* out, uint32_t ntiles, size_t smem, cudaStream_t stream)
 {
     if (getenv("SPPARK_B200_NTT_GENERIC")) return false;
-    // 256-bit fields run the run-time shaped kernel: their static twins were measured in round 2
-    // (shapes of 2^20, 2^22, 2^24) at 9 % faster for a 9-minute compile of this translation unit;
+    // 256-bit fields run the run-time shaped kernel: static twins (shapes of 2^20, 2^22, 2^24) cost
+    // a 9-minute compile of this translation unit for a small gain on the GPU this was tuned on;
     // the kernel's cost is elsewhere (DESIGN.md section 4.4)
     if constexpr (F::LG_EPT != 4) return false;
     else return try_shapes<F, 12, 2>(d, tb, in, out, ntiles, smem, stream)

@@ -265,9 +265,9 @@ private:
     }
 
     // Which pass kernel: below 2^20 elements the warp-autonomous passes (ntt_warp.cuh: no block
-    // barrier, any number of warps busy) win -- 2^16: 23 us against 37 us; from 2^20 on the two
-    // 12-stage block-tile passes move a third less data and are ahead by 5-10 % (B200, round 2:
-    // gpurun_out/r2_probe_ntt6.txt, summarised in profiles/).  SPPARK_B200_NTT_WARP=1 /
+    // barrier, any number of warps busy) win; from 2^20 on the two 12-stage block-tile passes move
+    // a third less data (the crossover was chosen on an earlier GPU and has not been re-measured
+    // on H100).  SPPARK_B200_NTT_WARP=1 /
     // SPPARK_B200_NTT_BLOCK=1 force one or the other (experiments, tests).
     static bool use_warp_path(uint32_t lg_n)
     {
@@ -305,7 +305,7 @@ public:
             lg_tile = WARP_MAX_LG_R + 6;                  // up to 64 adjacent columns per tile
         } else {
             // 2^14-element tiles fill one SM's shared memory; below 2^22 elements shrink the tile so
-            // that there are still >= 256 of them for the 148 SMs
+            // that there are still >= 256 of them for the 132 SMs
             if (lg_n < lg_tile + 8) lg_tile = lg_n > 18 ? lg_n - 8 : 10;
             if (const char* env = getenv("SPPARK_B200_NTT_LG_TILE")) lg_tile = (uint32_t)atoi(env);
             if (lg_tile > FieldId<F>::lg_tile) lg_tile = FieldId<F>::lg_tile;

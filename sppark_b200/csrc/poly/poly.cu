@@ -95,7 +95,7 @@ static void scan(const gpu_t& gpu, cudaStream_t stream, typename F::T* out, cons
         COUNT_LAUNCH();
         CUDA_OK(cudaGetLastError());
         // the aggregates' own scan: a few tiles; one CTA walking them serially is a chain of ~25 dependent
-        // joins per tile (BLS12-381 fr 2^22: 81 us for 4 tiles), so beyond two tiles they run side by side
+        // joins per tile, so beyond two tiles they run side by side
         const uint32_t nagg_tiles = (uint32_t)((ntiles + TILE - 1) / TILE);
         if (!(nagg_tiles > 2 && nagg_tiles <= scan_capacity<F, OP, MODE_COOP, false>(gpu) &&
               try_coop([&] { scan_launch<F, OP, MODE_COOP, false>(gpu, stream, ~0u, aggs, aggs, ntiles, zt, 0, nagg_tiles, aggs2, nullptr); })))
@@ -157,8 +157,8 @@ static void batch_inverse(const gpu_t& gpu, cudaStream_t stream, typename F::T* 
     const size_t nchunks = (len + (size_t)IBS * N - 1) / ((size_t)IBS * N);
     const uint32_t grid = (uint32_t)std::min<size_t>(nchunks, (size_t)gpu.sm_count() * 8);
     // one inversion per chunk inside the kernel: always for the word fields (their inversion is ~100 short
-    // multiplications; hoisting it measured slower, BabyBear 2^24: 127 us against 98 us), and for the wide
-    // fields while every chunk has an SM to itself (BLS12-381 fr 2^16: 249 us against 327 us hoisted)
+    // multiplications; hoisting it measured slower on the GPU this was tuned on), and for the wide
+    // fields while every chunk has an SM to itself
     if (!wide || nchunks <= 2 * (size_t)gpu.sm_count()) {
         batch_inverse_kernel<F, N, IBS, INV_SELF><<<grid, IBS, 0, stream>>>(d_out, d_inp, len, nullptr);
         COUNT_LAUNCH();

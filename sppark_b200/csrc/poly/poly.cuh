@@ -227,9 +227,9 @@ DEV typename F::T block_wreduce(typename F::T val, const typename F::T& base, ty
 //   tile_reduce_kernel        every tile's aggregate -> aggs[tile]                      (reads the data once)
 //   scan_kernel MODE_SERIAL   ONE CTA scans aggs[] in place, tile after tile            (ntiles elements)
 //   scan_kernel MODE_SCAN     every tile rescanned with carry aggs[tile-1] and stored   (reads + writes the data)
-// A decoupled look-back single pass was measured first and rejected: its carry chain advances at
-// most one 32-tile window per L2 round trip, which capped 2^24 Goldilocks elements at 230 us where
-// these three launches are bandwidth bound (profiles/poly_r02.md).  Short inputs take MODE_SERIAL
+// A decoupled look-back single pass was tried first and rejected: its carry chain advances at most
+// one 32-tile window per L2 round trip, where these three launches are bandwidth bound.  Short
+// inputs take MODE_SERIAL
 // directly on the data (one launch).  Inputs whose tiles are all resident at once take MODE_COOP:
 // one cooperative launch, one tile per CTA kept in registers across a single grid barrier, after
 // which every CTA folds the aggregates of the tiles before it by itself (a few KB from L2) -- one

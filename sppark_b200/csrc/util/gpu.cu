@@ -1,6 +1,7 @@
 // Device enumeration: the reference's util/all_gpus.cpp:14-63 (gpus_t, select_gpu, ngpus,
-// all_gpus) for this library.  Requires compute capability 10.x (the kernels are sm_100a
-// only); anything else is treated as "no device", there is no fallback path.
+// all_gpus) for this library.  Requires compute capability 9.0 (the kernels are built for
+// sm_90a only, which loads on no other architecture); anything else is treated as "no device",
+// there is no fallback path.
 #include "gpu.cuh"
 
 namespace {
@@ -14,7 +15,7 @@ struct gpus_t {
         (void)cudaGetDevice(&prev);
         for (int id = 0; id < n; id++) {
             cudaDeviceProp prop;
-            if (cudaGetDeviceProperties(&prop, id) == cudaSuccess && prop.major == 10) {
+            if (cudaGetDeviceProperties(&prop, id) == cudaSuccess && prop.major == 9 && prop.minor == 0) {
                 try { gpus.push_back(new gpu_t((int)gpus.size(), id)); } catch (const cuda_error&) {}
             }
         }
@@ -35,7 +36,7 @@ const gpu_t& gpu_of_current_device()
     CUDA_OK(cudaGetDevice(&cid));
     for (auto* g : gpus)
         if (g->cid() == cid) return *g;
-    throw cuda_error(-(int)cudaErrorInvalidDevice, "current CUDA device is not a B200-class (sm_100) device");
+    throw cuda_error(-(int)cudaErrorInvalidDevice, "current CUDA device is not an H100-class (sm_90) device");
 }
 
 const gpu_t& select_gpu(int id)

@@ -1,6 +1,6 @@
 // Host/device portability macros.  Every arithmetic and index-mapping routine of the
 // hot path is written HD so that tests/emu/*.cpp can single-step the exact kernel logic
-// on the CPU (phase by phase) before it is run on a B200.  The product path itself is
+// on the CPU (phase by phase) before it is run on the GPU.  The product path itself is
 // CUDA only: nothing here provides a CPU fallback for the C-ABI entry points.
 #pragma once
 #include <cstddef>

@@ -1,9 +1,5 @@
 """Builds the C++-layer test programs (tests/test_cpp_layer.py, __graft_entry__.build()):
   _build/dropin_example        tests/cpp/dropin_example.cpp against include/sppark_b200.hpp
-  _build/libdropin_*.so        THE REFERENCE'S OWN poc glue (poc/msm-cuda/cuda/pippenger.cu,
-                               pippenger_inf.cu, poc/ntt-cuda/cuda/ntt_api.cu), compiled unmodified
-                               from where it lies against include/compat/ with plain g++ -- only
-                               where /root/reference exists; the .so files travel to the GPU box.
 """
 import os
 import subprocess
@@ -11,19 +7,8 @@ import subprocess
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 OUT = os.path.join(HERE, "_build")
-REF = "/root/reference"
-CUDA_INC = "/usr/local/cuda/include"           # <cuda.h> only: the glue includes it, uses nothing of it
 LINK = ["-L" + os.path.join(ROOT, "sppark_b200"), "-lsppark_b200", "-Wl,-rpath," + os.path.join(ROOT, "sppark_b200"),
         "-Wl,-rpath,$ORIGIN/../../../sppark_b200"]
-
-GLUE = [("libdropin_msm_g1.so", "poc/msm-cuda/cuda/pippenger.cu", "FEATURE_BLS12_381"),
-        ("libdropin_msm.so", "poc/msm-cuda/cuda/pippenger_inf.cu", "FEATURE_BLS12_381"),
-        ("libdropin_ntt_gl64.so", "poc/ntt-cuda/cuda/ntt_api.cu", "FEATURE_GOLDILOCKS"),
-        ("libdropin_ntt_bb31.so", "poc/ntt-cuda/cuda/ntt_api.cu", "FEATURE_BABY_BEAR"),
-        ("libdropin_ntt_bls12_381.so", "poc/ntt-cuda/cuda/ntt_api.cu", "FEATURE_BLS12_381"),
-        ("libdropin_msm_bn254.so", "poc/msm-cuda/cuda/pippenger_inf.cu", "FEATURE_BN254"),
-        ("libdropin_msm_bls12_377.so", "poc/msm-cuda/cuda/pippenger_inf.cu", "FEATURE_BLS12_377")]
-
 
 def build_example():
     os.makedirs(OUT, exist_ok=True)
@@ -36,20 +21,5 @@ def build_example():
     return exe, exe_ntt
 
 
-def build_reference_glue():
-    """-> list of built libraries ([] when the reference is not on this machine)."""
-    if not os.path.isdir(REF):
-        return []
-    os.makedirs(OUT, exist_ok=True)
-    built = []
-    for name, src, feature in GLUE:
-        out = os.path.join(OUT, name)
-        subprocess.check_call(["g++", "-std=c++17", "-x", "c++", "-D" + feature, "-I" + os.path.join(ROOT, "include", "compat"),
-                               "-I" + CUDA_INC, "-fPIC", "-shared", "-o", out, os.path.join(REF, src), *LINK])
-        built.append(out)
-    return built
-
-
 if __name__ == "__main__":
     print(build_example())
-    print(build_reference_glue())

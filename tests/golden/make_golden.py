@@ -1,9 +1,9 @@
 """Generates the committed golden vectors from THE REFERENCE ITSELF (not from the oracle):
 
   ntt_ref_gpu.npz   inputs/outputs of the reference's own CUDA NTT (poc/ntt-cuda/cuda/ntt_api.cu
-                    compiled for sm_100a into oracle/_ref by oracle/Makefile), Goldilocks and
-                    BabyBear, lg 1..10, every order x direction x type.  Needs a GPU: run as
-                    `gpurun -- python tests/golden/make_golden.py gpu` and copy gpurun_out/golden/*.
+                    compiled for sm_90a into oracle/_ref by oracle/Makefile), Goldilocks and
+                    BabyBear, lg 1..10, every order x direction x type.  Needs a GPU:
+                    `python tests/golden/make_golden.py gpu`, then copy the files it wrote here.
   msm_ref_gpu.npz   same for the reference's CUDA mult_pippenger (BLS12-381 G1).
   msm_g2_ref_gpu.npz  the reference's mult_pippenger_fp2_inf (BLS12-381 G2) and mult_pippenger_inf
                     (G1, arkworks layout with infinity flags): `... make_golden.py g2` on a GPU.
@@ -15,9 +15,16 @@
                     evaluate) through oracle/ref_poly.cu: `... make_golden.py poly_gl64|poly_bb31|poly_bls12_381_fr`.
   msm_ref_cpu.npz   the reference's CPU msm/pippenger.hpp (oracle/_ref/libref_msm_cpu.so);
                     runs anywhere: `python tests/golden/make_golden.py cpu`.
+  msm_ref_cpu_live.npz  the same CPU build on the 700-point case of tests/test_oracle.py:
+                    `python tests/golden/make_golden.py cpu_live`.
+  msm_2pow26_ref_gpu.npz  the reference's CUDA mult_pippenger on the 2^26-point instance of
+                    tests/test_msm_gpu.py (affine result only): `... make_golden.py msm_2pow26` on a GPU.
+  ref_params.json   the parameter tables the reference hard-codes (NTT roots of unity, Montgomery
+                    constants), parsed from its headers: `python tests/golden/make_golden.py params <reference tree>`.
 
 tests/test_oracle.py checks the CPU oracle against all three, which is what pins it.
-Inputs are seeded; nothing here reads /root/reference at run time (only the prebuilt _ref .so).
+Inputs are seeded; nothing here reads the reference's sources at run time (only the prebuilt _ref
+.so), except `params`, which parses its headers.
 """
 import ctypes as C
 import os
@@ -74,6 +81,101 @@ def gen_cpu(outdir):
         out[f"affine_{n}"] = o.jac_to_affine("bls12_381", jac)
     np.savez_compressed(os.path.join(outdir, "msm_ref_cpu.npz"), **out)
     print("wrote msm_ref_cpu.npz")
+
+
+def gen_cpu_live(outdir):
+    """the inputs of tests/test_oracle.py::test_oracle_matches_reference_cpu_live"""
+    n = 700
+    import random
+    pts = o.gen_points("bls12_381", 50)[np.arange(n) % 50].copy()
+    rnd = random.Random(3)
+    sc = np.array([o.int_to_limbs(rnd.randrange(R_BLS), 4) for _ in range(n)], dtype=np.uint64)
+    affine = o.jac_to_affine("bls12_381", o.ref_cpu_msm(pts, sc, nthreads=4))
+    np.savez_compressed(os.path.join(outdir, "msm_ref_cpu_live.npz"), sc=sc, affine=affine)
+    print("wrote msm_ref_cpu_live.npz")
+
+
+def msm_2pow26_inputs(base):
+    """2^26 points replicating `base` (2^16 distinct), scalars uniform below 2^254 from seed 26"""
+    n, m = 1 << 26, base.shape[0]
+    pts = np.empty((n, 12), dtype=np.uint64)
+    pts.reshape(n // m, m, 12)[:] = base
+    rng = np.random.default_rng(26)
+    sc = np.empty((n, 4), dtype=np.uint64)
+    for s in range(0, n, 1 << 22):
+        sc[s:s + (1 << 22)] = rng.integers(0, 2**64, size=(1 << 22, 4), dtype=np.uint64)
+    sc[:, 3] >>= np.uint64(2)
+    return pts, sc
+
+
+def gen_msm_2pow26(outdir):
+    lib = C.CDLL(o.ref_path("libref_msm_gpu.so"))
+    lib.mult_pippenger.restype = RE
+    lib.mult_pippenger.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+    pts, sc = msm_2pow26_inputs(o.gen_points("bls12_381", 1 << 16))
+    jac = np.zeros(18, dtype=np.uint64)
+    ok(lib.mult_pippenger(jac.ctypes.data, pts.ctypes.data, pts.shape[0], sc.ctypes.data), "mult_pippenger")
+    np.savez_compressed(os.path.join(outdir, "msm_2pow26_ref_gpu.npz"), affine=o.jac_to_affine("bls12_381", jac))
+    print("wrote msm_2pow26_ref_gpu.npz")
+
+
+def gen_params(outdir, ref):
+    """ref_params.json: the tables of ntt/parameters/*.h and the device constants of ff/*.hpp,
+    as numbers (hex strings), for tests/test_params_pin.py"""
+    import json
+    import re
+
+    def small_table(path, name):
+        s = open(path).read()
+        tail = s.split("#endif")[-1]
+        if "#else" in s:
+            s = s.split("#else")[1].split("#endif")[0]
+        m = re.search(r"const fr_t %s\[S \+ 1\] = \{(.*?)\};" % name, s + tail, re.S)
+        return [int(x, 16) for x in re.findall(r"fr_t\((0x[0-9a-f]+)u?\)", m.group(1))]
+
+    def device_words(path, name):
+        s = open(path).read().split("namespace device")[1]
+        m = re.search(r"%s\[\d+\] = \{(.*?)\};" % name, s, re.S)
+        words = []
+        for v in re.findall(r"TO_CUDA_T\((0x[0-9a-f]+)\)", m.group(1)):
+            v = int(v, 16)
+            words += [v & 0xFFFFFFFF, v >> 32]
+        if not words:                                   # pasta.hpp lists plain 32-bit words
+            words = [int(v, 16) for v in re.findall(r"0x[0-9a-f]{8}", m.group(1))]
+        return words
+
+    def wide_table(path):
+        s = open(path).read()
+        out = {}
+        for m in re.finditer(r"const fr_t (\w+)\[S \+ 1\] = \{(.*?)\};", s, re.S):
+            vals = []
+            for mm in re.finditer(r"FR_T\(vec256,(.*?)\)", m.group(2)):
+                limbs = [int(x.strip().rstrip("u"), 16) for x in mm.group(1).split(",")]
+                vals.append(sum(v << (64 * i) for i, v in enumerate(limbs)))
+            out[m.group(1)] = vals
+        m = re.search(r"const fr_t group_gen = FR_T\(vec256,(.*?)\)", s)
+        limbs = [int(x.strip().rstrip("u"), 16) for x in m.group(1).split(",")]
+        out["group_gen"] = sum(v << (64 * i) for i, v in enumerate(limbs))
+        return out
+
+    hexify = lambda v: [hex(x) for x in v] if isinstance(v, list) else hex(v)   # noqa: E731
+    out = {"ntt_small": {}, "ntt_wide": {}, "device": {}}
+    for f in ("goldilocks", "baby_bear"):
+        out["ntt_small"][f] = {n: hexify(small_table(f"{ref}/ntt/parameters/{f}.h", n))
+                               for n in ("forward_roots_of_unity", "inverse_roots_of_unity", "domain_size_inverse")}
+    for f in ("bls12_381", "vesta", "pallas", "alt_bn128", "bls12_377"):
+        t = wide_table(f"{ref}/ntt/parameters/{f}.h")
+        out["ntt_wide"][f] = {k: hexify(t[k]) for k in ("group_gen", "forward_roots_of_unity", "domain_size_inverse")}
+    for hdr, names in (("bls12-381", ("BLS12_381_P", "BLS12_381_RR", "BLS12_381_one", "BLS12_381_r", "BLS12_381_rone")),
+                       ("pasta", ("Pallas_P", "Pallas_RR", "Pallas_one", "Vesta_P", "Vesta_RR", "Vesta_one")),
+                       ("alt_bn128", ("ALT_BN128_P", "ALT_BN128_RR", "ALT_BN128_one", "ALT_BN128_r", "ALT_BN128_rRR", "ALT_BN128_rone")),
+                       ("bls12-377", ("BLS12_377_P", "BLS12_377_RR", "BLS12_377_one", "BLS12_377_r", "BLS12_377_rone"))):
+        for name in names:
+            out["device"][name] = hexify(device_words(f"{ref}/ff/{hdr}.hpp", name))
+    with open(os.path.join(outdir, "ref_params.json"), "w") as f:
+        json.dump(out, f, indent=1)
+        f.write("\n")
+    print("wrote ref_params.json")
 
 
 # Every reference library is loaded in a process of its own: the reference's NTT keeps its
@@ -138,8 +240,19 @@ def gen_ntt256(outdir):
                     e = lib.compute_ntt(0, y.ctypes.data, lg, order, direction, typ)
                     assert e.code == 0
                     out[f"out_{lg}_{order}{direction}{typ}"] = y
-    np.savez_compressed(os.path.join(outdir, "ntt256_ref_gpu.npz"), **out)
+    np.savez_compressed(os.path.join(outdir, "ntt256_ref_gpu.npz"), **sample_ntt256(out))
     print("wrote ntt256_ref_gpu.npz")
+
+
+def sample_ntt256(out, lg=10, k=512):
+    """keeps the file under 1 MB: of the 2^lg-point outputs only k rows, a fixed seeded sample
+    (stored as rows_<lg>), are kept; the input stays whole"""
+    rows = np.sort(np.random.default_rng(256).choice(1 << lg, size=k, replace=False))
+    out = dict(out)
+    out[f"rows_{lg}"] = rows
+    for key in [k_ for k_ in out if k_.startswith(f"out_{lg}_")]:
+        out[key] = out[key][rows]
+    return out
 
 
 def gen_msm(outdir):
@@ -197,7 +310,7 @@ def g2_inputs():
 
 def gen_g2(outdir):
     """msm_g2_ref_gpu.npz: the reference's mult_pippenger_fp2_inf (and, for the G1 arkworks layout,
-    mult_pippenger_inf) from oracle/_ref/libref_msm_g2_gpu.so, run on a B200."""
+    mult_pippenger_inf) from oracle/_ref/libref_msm_g2_gpu.so, run on a GPU."""
     lib = C.CDLL(o.ref_path("libref_msm_g2_gpu.so"))
     for f in (lib.mult_pippenger_fp2_inf, lib.mult_pippenger_inf):
         f.restype = RE
@@ -307,7 +420,7 @@ def gen_pasta(outdir):
 def gen_poly(outdir, field):
     """poly_<field>_ref_gpu.npz: the reference's polynomial/ templates (oracle/ref_poly.cu) on
     seeded inputs in the field's memory format.  One reference library per process.  Two limits
-    of the reference itself are stepped around (profiles/ref_poly_probe_r02.txt): its evaluate
+    of the reference itself are stepped around: its evaluate
     faults at len = 1, and its 256-bit div_by_x_minus_z faults for len <= 5001 -- those cases are
     not recorded.  The `big` case keeps SHA-256 digests of the outputs instead of the arrays; its
     input is regenerated from the seed by oracle.poly.seeded_input."""
@@ -412,6 +525,10 @@ if __name__ == "__main__":
     mode = sys.argv[1] if len(sys.argv) > 1 else "cpu"
     if mode == "cpu":
         gen_cpu(HERE)
+    elif mode == "cpu_live":
+        gen_cpu_live(HERE)
+    elif mode == "params":
+        gen_params(HERE, sys.argv[2])
     else:
         outdir = os.path.join(ROOT, "gpurun_out", "golden")
         os.makedirs(outdir, exist_ok=True)
@@ -429,6 +546,8 @@ if __name__ == "__main__":
             gen_ntt256(outdir)
         elif mode == "msm":
             gen_msm(outdir)
+        elif mode == "msm_2pow26":
+            gen_msm_2pow26(outdir)
         elif mode in ("g2_bn254", "g2_bls12_377"):
             gen_g2_curve(outdir, mode[3:])
         elif mode.startswith("poly_"):

@@ -1,6 +1,6 @@
 """world_size-2 (and 3) CPU runs of the multi-GPU host logic over the gloo backend: sharding,
 all-gather of partial results, folding.  The per-rank MSM is the CPU oracle here (there is no GPU
-in this tier); on the GPU box the same `parallel.msm_sharded` drives `sppark_b200_msm_dev` and
+in this tier); on a GPU machine the same `parallel.msm_sharded` drives `sppark_b200_msm_dev` and
 `sppark_b200_msm_combine` (bench.py --gpus N)."""
 import os
 import socket

@@ -114,7 +114,7 @@ def test_g2_packed_dev_generate_combine(oracle):
 
 def test_g2_matches_reference_gpu_golden(oracle):
     """Same group element as the reference's own mult_pippenger_fp2_inf / mult_pippenger_inf
-    recorded on a B200 (tests/golden/make_golden.py g2)."""
+    recorded from its CUDA build (tests/golden/make_golden.py g2)."""
     from sppark_b200 import msm
     path = os.path.join(os.path.dirname(__file__), "golden", "msm_g2_ref_gpu.npz")
     if not os.path.exists(path):

@@ -108,7 +108,7 @@ def test_bad_arguments_return_errors():
 
 
 def test_matches_reference_gpu_golden():
-    """Bit-exact against outputs of the reference's own CUDA NTT recorded on a B200
+    """Bit-exact against outputs of the reference's own CUDA NTT as recorded
     (tests/golden/ntt_ref_gpu.npz, made by tests/golden/make_golden.py): every order x direction
     x type; Goldilocks lg 1..10 through compute_ntt, BabyBear lg 1..12 through sppark_b200_ntt."""
     import os
@@ -191,18 +191,19 @@ def test_ntt_256bit_fields_match_oracle(oracle, fid, name):
 
 def test_ntt_256bit_matches_reference_gpu_golden():
     """BLS12-381 scalar field, lg 1..10, every order x direction x type, against the recording of
-    the reference's own 256-bit ("wide") CUDA kernels."""
+    the reference's own 256-bit ("wide") CUDA kernels (at lg 10, on the recorded sample of rows)."""
     import os
     from sppark_b200 import ntt
     g = np.load(os.path.join(os.path.dirname(__file__), "golden", "ntt256_ref_gpu.npz"))
     for lg in range(1, 11):
         x = g[f"in_{lg}"]
+        rows = g[f"rows_{lg}"] if f"rows_{lg}" in g.files else slice(None)
         for order in range(4):
             for d in range(2):
                 for t in range(2):
                     y = x.copy()
                     ntt._run(0, y, order, d, t, field=ntt.BLS12_381_FR)
-                    assert np.array_equal(y, g[f"out_{lg}_{order}{d}{t}"]), (lg, order, d, t)
+                    assert np.array_equal(y[rows], g[f"out_{lg}_{order}{d}{t}"]), (lg, order, d, t)
 
 
 def test_ntt_256bit_2pow22_roundtrip():

@@ -1,5 +1,5 @@
 """CPU: the G2 oracle (oracle/ec2.c) against an independent big-integer model and against the
-golden vectors recorded from the reference's mult_pippenger_fp2_inf on a B200."""
+golden vectors recorded from the reference's mult_pippenger_fp2_inf on a GPU."""
 import os
 import random
 
@@ -178,7 +178,7 @@ def test_g2_oracle_matches_reference_gpu_golden(oracle):
 
 def test_reference_fp2_inf_entry_is_inconsistent(oracle):
     """Documents why the pin above is taken on packed points (oracle/ref_msm_g2.cu): the reference's
-    own mult_pippenger_fp2_inf, built for sm_100a, agrees with its packed instantiation only for
+    own mult_pippenger_fp2_inf, as built with nvcc, agrees with its packed instantiation only for
     n = 1; for n = 2 it returns s0*P0 (point 1 is read at the wrong pitch and taken for infinity)."""
     path = os.path.join(HERE, "golden", "msm_g2_ref_gpu.npz")
     if not os.path.exists(path):

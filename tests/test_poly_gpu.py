@@ -34,7 +34,7 @@ def _sha(a):
 @pytest.mark.parametrize("field", ["gl64", "bb31", "bls12_381_fr"])
 def test_matches_the_reference_recordings(field):
     """every input/output pair tests/golden/make_golden.py recorded from the reference's own
-    kernels on a B200 (what the reference cannot run -- see gen_poly -- is absent from the file);
+    kernels (what the reference cannot run -- see gen_poly -- is absent from the file);
     the `big` case is compared through SHA-256 digests of whole output arrays"""
     from oracle import poly as op
     from sppark_b200 import poly

@@ -1,5 +1,5 @@
 """CPU: oracle/poly.py against the recordings of the reference's own polynomial kernels
-(tests/golden/poly_*_ref_gpu.npz, generated on a B200 by tests/golden/make_golden.py gen_poly
+(tests/golden/poly_*_ref_gpu.npz, generated on a GPU by tests/golden/make_golden.py gen_poly
 through oracle/ref_poly.cu) -- this is what pins the oracle the GPU parity tests rely on."""
 import hashlib
 import os

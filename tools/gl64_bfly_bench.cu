@@ -1,8 +1,8 @@
 // Compute-only microbenchmark of the Goldilocks butterfly network (no memory traffic): which
-// formulation of add / sub / mul issues fastest on a B200, and what IPC a dense stream of them
+// formulation of add / sub / mul issues fastest on the GPU, and what IPC a dense stream of them
 // reaches.  One 16-point DFT = 32 butterflies (17 with a constant multiplication) on registers,
 // the code of ntt_warp.cuh's dft_stage, repeated ITER times per thread.
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -I sppark_b200/csrc -o /tmp/gl64_bfly tools/gl64_bfly_bench.cu
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -I sppark_b200/csrc -o /tmp/gl64_bfly tools/gl64_bfly_bench.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -1,6 +1,6 @@
-// Integer-issue microbenchmark for B200: what bounds the 384-bit Montgomery ladders?
+// Integer-issue microbenchmark: what bounds the 384-bit Montgomery ladders?
 // Measures warp-instruction throughput of IMAD.WIDE.U32 carry chains (the MSM inner loop),
-// plain IMAD, and IADD3, per SM per clock.   nvcc -arch=sm_100a -O3 imad_bench.cu -o imad_bench
+// plain IMAD, and IADD3, per SM per clock.   nvcc -arch=sm_90a -O3 imad_bench.cu -o imad_bench
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-"""Summarise an .ncu-rep (from `ncu --set full`) into a small markdown table for profiles/.
+"""Summarise an .ncu-rep (from `ncu --set full`) into a small markdown table.
 usage: ncu_summary.py REPORT.ncu-rep OUT.md "title" """
 import csv, subprocess, sys
 

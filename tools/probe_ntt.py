@@ -1,5 +1,5 @@
 """GPU probe: time our NTT (device-resident) against the reference's own kernels built for
-sm_100a (oracle/_ref), over the kernel variants selected by environment knobs.  Two clocks per
+sm_90a (oracle/_ref), over the kernel variants selected by environment knobs.  Two clocks per
 case: `call` = one call between two events (includes the host-side launch path while the GPU is
 idle), `b2b` = 20 calls back to back divided by 20 (the GPU never waits for the host: kernel time).
 Development tool, not the bench."""

@@ -1,5 +1,5 @@
 """GPU probe (test infrastructure): which build of the REFERENCE's BabyBear / 256-bit NTT is
-self-consistent on this B200?  oracle/Makefile `ref-variants` builds, next to the sm_100a SASS
+self-consistent on this GPU?  oracle/Makefile `ref-variants` builds, next to the sm_90a SASS
 libraries, a PTX-only one (what the crate ships: rust/src/build.rs:54-57, JIT on the device) and
 one with un-optimised device code.  For every library: the reference's own protocol
 (poc/ntt-cuda/tests/ntt.rs: NN == RR, iNTT(NTT(x)) == x, NR -> RN round trip) and equality with
