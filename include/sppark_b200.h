@@ -145,6 +145,25 @@ RustError sppark_b200_lde_powers_dev(int field, void *d_inout, uint32_t lg_domai
 RustError sppark_b200_lde_expand_dev(int field, void *d_out, const void *d_in, uint32_t lg_domain_size,
                                      uint32_t lg_blowup, void *stream);
 
+/* Batched NTT and LDE (the reference has no batched entry): `batch` transforms of 2^lg elements
+ * each, stored one after another (row b = elements [b * 2^lg, (b + 1) * 2^lg)) in the field's memory
+ * format.  Every row comes out exactly as the single-transform entry with the same order, direction
+ * and type returns it.  lg == 0 or batch == 0 is a no-op; a byte size that overflows size_t is
+ * rejected before any memory is touched.
+ *   ntt_batch_dev: device memory, in place, enqueued on `stream`, not synchronised;
+ *   lde_batch_dev: d_in = batch x 2^lg evaluations, overwritten with each row's coefficients in
+ *                  bit-reversed order; d_out = batch x 2^(lg + lg_blowup) evaluations on the coset,
+ *                  natural order (per row what sppark_b200_lde returns); the two must not overlap;
+ *                  enqueued on `stream`;
+ *   ntt_batch:     host memory, in place, synchronised; groups of rows are uploaded, transformed and
+ *                  downloaded in a pipeline (pinned or registered memory overlaps copies and work). */
+RustError sppark_b200_ntt_batch_dev(int field, void *d_inout, uint32_t lg_domain_size, size_t batch,
+                                    int ntt_order, int ntt_direction, int ntt_type, void *stream);
+RustError sppark_b200_lde_batch_dev(int field, void *d_out, void *d_in, uint32_t lg_domain_size,
+                                    uint32_t lg_blowup, size_t batch, void *stream);
+RustError sppark_b200_ntt_batch(int field, size_t device_id, void *inout, uint32_t lg_domain_size,
+                                size_t batch, int ntt_order, int ntt_direction, int ntt_type);
+
 /* ---- polynomial helpers (SURVEY.md section 8, row f4) ----------------------------------------------
  * The reference's polynomial/ templates and ff/batch_inversion.hpp for the NTT fields above.  All
  * arrays are DEVICE memory in the field's memory format (the format compute_ntt uses), the work is

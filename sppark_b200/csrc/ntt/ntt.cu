@@ -136,6 +136,59 @@ static RustError ntt_dev(void* d_inout, uint32_t lg, int order, int direction, i
 }
 
 template<class F>
+static RustError ntt_batch_host(size_t device_id, void* inout, uint32_t lg, size_t batch, int order, int direction,
+                                int type)
+{
+    typedef ntt::NTT<F> N;
+    if (order < 0 || order > 4 || direction < 0 || direction > 1 || type < 0 || type > 1)
+        return rust_err(-(int)cudaErrorInvalidValue, "ntt_batch: bad order/direction/type");
+    try {
+        const gpu_t& gpu = select_gpu((int)device_id);
+        return N::Base_batch(gpu, (typename F::T*)inout, lg, batch, (typename N::InputOutputOrder)order,
+                             (typename N::Direction)direction, (typename N::Type)type);
+    } catch (const cuda_error& e) {
+        return rust_err(e.code(), e.what());
+    } catch (const std::exception& e) {
+        return rust_err(-1, e.what());
+    }
+}
+
+template<class F>
+static RustError ntt_batch_dev(void* d_inout, uint32_t lg, size_t batch, int order, int direction, int type,
+                               void* stream)
+{
+    typedef ntt::NTT<F> N;
+    if (order < 0 || order > 4 || direction < 0 || direction > 1 || type < 0 || type > 1)
+        return rust_err(-(int)cudaErrorInvalidValue, "ntt_batch_dev: bad order/direction/type");
+    if (lg > (uint32_t)F::MAX_LG || !N::batch_fits(lg, batch))
+        return rust_err(-(int)cudaErrorInvalidValue, "ntt_batch_dev: lg_domain_size or batch out of range for this field");
+    try {
+        const gpu_t& gpu = gpu_of_current_device();
+        N::NTT_internal(gpu, (typename F::T*)d_inout, lg, (typename N::InputOutputOrder)order,
+                        (typename N::Direction)direction, (typename N::Type)type, (cudaStream_t)stream, batch);
+        return rust_ok();
+    } catch (const cuda_error& e) {
+        return rust_err(e.code(), e.what());
+    } catch (const std::exception& e) {
+        return rust_err(-1, e.what());
+    }
+}
+
+template<class F>
+static RustError lde_batch_dev(void* d_out, void* d_in, uint32_t lg, uint32_t lg_blowup, size_t batch, void* stream)
+{
+    try {
+        ntt::NTT<F>::LDE_batch_dev(gpu_of_current_device(), (cudaStream_t)stream, (typename F::T*)d_out,
+                                   (typename F::T*)d_in, lg, lg_blowup, batch);
+        return rust_ok();
+    } catch (const cuda_error& e) {
+        return rust_err(e.code(), e.what());
+    } catch (const std::exception& e) {
+        return rust_err(-1, e.what());
+    }
+}
+
+template<class F>
 static RustError ntt_slab(int which, const void* d_in, void* d_out, uint32_t lg, uint32_t lg_g, uint32_t rank,
                           int direction, void* stream, void* const* peers = nullptr)
 {
@@ -415,5 +468,50 @@ extern "C" RustError sppark_b200_ntt_dev(int field, void* d_inout, uint32_t lg, 
     case SPPARK_FIELD_BN254_FR: return ntt_dev<ff::bn254_fr_ntt>(d_inout, lg, order, direction, type, stream);
     case SPPARK_FIELD_BLS12_377_FR: return ntt_dev<ff::bls12_377_fr_ntt>(d_inout, lg, order, direction, type, stream);
     default: return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_ntt_dev: unknown field");
+    }
+}
+
+extern "C" RustError sppark_b200_ntt_batch_dev(int field, void* d_inout, uint32_t lg, size_t batch, int order,
+                                               int direction, int type, void* stream)
+{
+    switch (field) {
+    case SPPARK_FIELD_GL64: return ntt_batch_dev<gl64>(d_inout, lg, batch, order, direction, type, stream);
+    case SPPARK_FIELD_BB31: return ntt_batch_dev<bb31>(d_inout, lg, batch, order, direction, type, stream);
+    case SPPARK_FIELD_BLS12_381_FR: return ntt_batch_dev<ff::bls12_381_fr_ntt>(d_inout, lg, batch, order, direction, type, stream);
+    case SPPARK_FIELD_PALLAS_FR: return ntt_batch_dev<ff::pallas_fr_ntt>(d_inout, lg, batch, order, direction, type, stream);
+    case SPPARK_FIELD_VESTA_FR: return ntt_batch_dev<ff::vesta_fr_ntt>(d_inout, lg, batch, order, direction, type, stream);
+    case SPPARK_FIELD_BN254_FR: return ntt_batch_dev<ff::bn254_fr_ntt>(d_inout, lg, batch, order, direction, type, stream);
+    case SPPARK_FIELD_BLS12_377_FR: return ntt_batch_dev<ff::bls12_377_fr_ntt>(d_inout, lg, batch, order, direction, type, stream);
+    default: return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_ntt_batch_dev: unknown field");
+    }
+}
+
+extern "C" RustError sppark_b200_lde_batch_dev(int field, void* d_out, void* d_in, uint32_t lg, uint32_t lg_blowup,
+                                               size_t batch, void* stream)
+{
+    switch (field) {
+    case SPPARK_FIELD_GL64: return lde_batch_dev<gl64>(d_out, d_in, lg, lg_blowup, batch, stream);
+    case SPPARK_FIELD_BB31: return lde_batch_dev<bb31>(d_out, d_in, lg, lg_blowup, batch, stream);
+    case SPPARK_FIELD_BLS12_381_FR: return lde_batch_dev<ff::bls12_381_fr_ntt>(d_out, d_in, lg, lg_blowup, batch, stream);
+    case SPPARK_FIELD_PALLAS_FR: return lde_batch_dev<ff::pallas_fr_ntt>(d_out, d_in, lg, lg_blowup, batch, stream);
+    case SPPARK_FIELD_VESTA_FR: return lde_batch_dev<ff::vesta_fr_ntt>(d_out, d_in, lg, lg_blowup, batch, stream);
+    case SPPARK_FIELD_BN254_FR: return lde_batch_dev<ff::bn254_fr_ntt>(d_out, d_in, lg, lg_blowup, batch, stream);
+    case SPPARK_FIELD_BLS12_377_FR: return lde_batch_dev<ff::bls12_377_fr_ntt>(d_out, d_in, lg, lg_blowup, batch, stream);
+    default: return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_lde_batch_dev: unknown field");
+    }
+}
+
+extern "C" RustError sppark_b200_ntt_batch(int field, size_t device_id, void* inout, uint32_t lg, size_t batch,
+                                           int order, int direction, int type)
+{
+    switch (field) {
+    case SPPARK_FIELD_GL64: return ntt_batch_host<gl64>(device_id, inout, lg, batch, order, direction, type);
+    case SPPARK_FIELD_BB31: return ntt_batch_host<bb31>(device_id, inout, lg, batch, order, direction, type);
+    case SPPARK_FIELD_BLS12_381_FR: return ntt_batch_host<ff::bls12_381_fr_ntt>(device_id, inout, lg, batch, order, direction, type);
+    case SPPARK_FIELD_PALLAS_FR: return ntt_batch_host<ff::pallas_fr_ntt>(device_id, inout, lg, batch, order, direction, type);
+    case SPPARK_FIELD_VESTA_FR: return ntt_batch_host<ff::vesta_fr_ntt>(device_id, inout, lg, batch, order, direction, type);
+    case SPPARK_FIELD_BN254_FR: return ntt_batch_host<ff::bn254_fr_ntt>(device_id, inout, lg, batch, order, direction, type);
+    case SPPARK_FIELD_BLS12_377_FR: return ntt_batch_host<ff::bls12_377_fr_ntt>(device_id, inout, lg, batch, order, direction, type);
+    default: return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_ntt_batch: unknown field");
     }
 }

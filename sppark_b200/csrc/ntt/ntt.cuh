@@ -127,21 +127,16 @@ __global__ void gen_coset_kernel(typename F::T* g0, typename F::T* g1, typename 
     if (i < 256) g2[i] = F::pow(g, (uint64_t)i << 24);
 }
 
+// over a batch of transforms of 2^lg_n elements each: `count` = batch << lg_n elements, the
+// exponent is taken within each transform
 template<class F>
 __global__ void coset_kernel(typename F::T* data, uint32_t lg_n, bool bitrev,
                              const typename F::T* g0, const typename F::T* g1,
-                             const typename F::T* g2)
+                             const typename F::T* g2, size_t count)
 {
-    typedef typename F::T T;
-    const size_t n = (size_t)1 << lg_n;
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n;
-         i += (size_t)gridDim.x * blockDim.x) {
-        uint32_t e = bitrev ? brev32((uint32_t)i, lg_n) : (uint32_t)i;
-        T x = F::mul(F::load(data[i]), g0[e & 4095]);
-        if (e >> 12) x = F::mul(x, g1[(e >> 12) & 4095]);
-        if (e >> 24) x = F::mul(x, g2[e >> 24]);
-        data[i] = F::canon(x);
-    }
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < count;
+         i += (size_t)gridDim.x * blockDim.x)
+        data[i] = F::canon(coset_mul<F>(F::load(data[i]), i, lg_n, bitrev, g0, g1, g2));
 }
 
 // LDE: zero-stuffing blow-up fused with the coset shift (reference:
@@ -161,22 +156,20 @@ __global__ void bitrev_copy_kernel(typename F::T* out, const typename F::T* in, 
 template<class F>
 __global__ void lde_spread_kernel(typename F::T* out, const typename F::T* in, uint32_t lg_n, uint32_t lg_blowup,
                                   const typename F::T* g0, const typename F::T* g1, const typename F::T* g2,
-                                  bool shift = true)
+                                  bool shift = true, size_t batch = 1)
 {
+    // a batch: `batch` rows of 2^lg_n in, rows of 2^(lg_n + lg_blowup) out; row r's slot i << lg_blowup
+    // is element (r << (lg_n + lg_blowup)) + (i << lg_blowup) = (global input index) << lg_blowup
     typedef typename F::T T;
-    const size_t n_ext = (size_t)1 << (lg_n + lg_blowup);
+    const size_t n_ext = batch << (lg_n + lg_blowup);
     const uint32_t mask = (1u << lg_blowup) - 1;
     T zero = F::sub(F::one(), F::one());
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n_ext; i += (size_t)gridDim.x * blockDim.x) {
         T x = zero;
         if ((i & mask) == 0) {
-            uint32_t src = (uint32_t)(i >> lg_blowup), e = brev32(src, lg_n);
+            const size_t src = i >> lg_blowup;
             x = F::load(in[src]);
-            if (shift) {
-                x = F::mul(x, g0[e & 4095]);
-                if (e >> 12) x = F::mul(x, g1[(e >> 12) & 4095]);
-                if (e >> 24) x = F::mul(x, g2[e >> 24]);
-            }
+            if (shift) x = coset_mul<F>(x, src, lg_n, true, g0, g1, g2);
             x = F::canon(x);
         }
         out[i] = x;
@@ -253,13 +246,13 @@ private:
     }
 
     static void coset_scale(const gpu_t& gpu, T* d_inout, uint32_t lg_n, bool bitrev, bool inverse,
-                            cudaStream_t stream)
+                            cudaStream_t stream, size_t batch = 1)
     {
         const CosetTables& ct = coset_tables(gpu, inverse, stream);
-        size_t n = (size_t)1 << lg_n;
-        uint32_t blocks = (uint32_t)((n + 255) / 256);
-        uint32_t cap = (uint32_t)gpu.sm_count() * 16;
-        coset_kernel<F><<<blocks < cap ? blocks : cap, 256, 0, stream>>>(d_inout, lg_n, bitrev, ct.g0, ct.g1, ct.g2);
+        size_t n = batch << lg_n;
+        size_t blocks = (n + 255) / 256;
+        size_t cap = (size_t)gpu.sm_count() * 16;
+        coset_kernel<F><<<(uint32_t)(blocks < cap ? blocks : cap), 256, 0, stream>>>(d_inout, lg_n, bitrev, ct.g0, ct.g1, ct.g2, n);
         COUNT_LAUNCH();
         CUDA_OK(cudaGetLastError());
     }
@@ -280,11 +273,13 @@ private:
     }
 
 public:
-    // device-resident transform, enqueued on `stream`, no synchronisation
+    // device-resident transform, enqueued on `stream`, no synchronisation.  batch > 1: `batch`
+    // transforms of 2^lg_n elements stored one after another, one plan and one launch per pass for
+    // all of them
     static void NTT_internal(const gpu_t& gpu, T* d_inout, uint32_t lg_n, InputOutputOrder order,
-                             Direction direction, Type type, cudaStream_t stream)
+                             Direction direction, Type type, cudaStream_t stream, size_t batch = 1)
     {
-        if (lg_n == 0) return;
+        if (lg_n == 0 || batch == 0) return;
         if (lg_n > (uint32_t)F::MAX_LG || lg_n > 30)
             throw cuda_error(-(int)cudaErrorInvalidValue, "NTT: lg_domain_size out of range");
         const bool inverse = direction == Direction::inverse;
@@ -293,10 +288,6 @@ public:
         const bool in_rev = order != InputOutputOrder::NN && order != InputOutputOrder::NR;
         const bool out_rev = order != InputOutputOrder::NN && order != InputOutputOrder::RN;
 
-        if (!inverse && type == Type::coset)
-            coset_scale(gpu, d_inout, lg_n, in_rev, false, stream);
-
-        const Tables<F>& tb = tables(gpu, lg_n, inverse, stream);
         // single-word fields: warp-autonomous passes of 2^4..2^8-point sub-NTTs (ntt_warp.cuh);
         // 256-bit fields (and SPPARK_B200_NTT_BLOCK=1): block-tile passes of up to 2^12 points
         const bool warp_path = use_warp_path(lg_n);
@@ -304,17 +295,33 @@ public:
         if (warp_path) {
             lg_tile = WARP_MAX_LG_R + 6;                  // up to 64 adjacent columns per tile
         } else {
-            // 2^14-element tiles fill one SM's shared memory; below 2^22 elements shrink the tile so
-            // that there are still >= 256 of them for the 132 SMs
-            if (lg_n < lg_tile + 8) lg_tile = lg_n > 18 ? lg_n - 8 : 10;
+            // 2^14-element tiles fill one SM's shared memory; below 2^22 elements (all transforms of
+            // a batch together) shrink the tile so that there are still >= 256 of them for the 132 SMs
+            uint32_t lg_total = lg_n;
+            while (lg_total < 63 && (batch >> (lg_total - lg_n)) > 1) lg_total++;   // floor(log2(batch << lg_n))
+            if (lg_total < lg_tile + 8) lg_tile = lg_total > 18 ? lg_total - 8 : 10;
             if (const char* env = getenv("SPPARK_B200_NTT_LG_TILE")) lg_tile = (uint32_t)atoi(env);
             if (lg_tile > FieldId<F>::lg_tile) lg_tile = FieldId<F>::lg_tile;
         }
         Plan plan = make_plan(lg_n, (int)order, inverse, lg_tile, 6, warp_path ? WARP_MAX_LG_R : F::NTT_MAX_LG_R);
+        if (batch > 1) {
+            if (!set_batch(plan, batch))
+                throw cuda_error(-(int)cudaErrorInvalidValue, "NTT: this plan cannot be batched");
+            // the tiles of the whole batch index one grid (the warp passes go in launches of < 2^31
+            // elements, below)
+            for (const Pass& d : plan.passes)
+                if ((batch << (lg_n - d.lg_r - d.lg_w)) > 0x7fffffffull)
+                    throw cuda_error(-(int)cudaErrorInvalidValue, "NTT: batch too large for this lg_domain_size");
+        }
+
+        if (!inverse && type == Type::coset)
+            coset_scale(gpu, d_inout, lg_n, in_rev, false, stream, batch);
+
+        const Tables<F>& tb = tables(gpu, lg_n, inverse, stream);
 
         T* scratch = nullptr;
         if (plan.needs_scratch)
-            CUDA_OK(cudaMallocAsync((void**)&scratch, sizeof(T) << lg_n, stream));
+            CUDA_OK(cudaMallocAsync((void**)&scratch, (sizeof(T) * batch) << lg_n, stream));
         T* buf[2] = {d_inout, scratch};
 
         static bool attr_done[64];
@@ -326,11 +333,22 @@ public:
         g_profile.reset();
         for (const Pass& d : plan.passes) {
             g_profile.mark("pass", stream);
-            uint32_t ntiles = 1u << (lg_n - d.lg_r - d.lg_w);
+            uint32_t ntiles = (uint32_t)(batch << (lg_n - d.lg_r - d.lg_w));
             size_t smem = smem_elems(d) * sizeof(T);
             bool done = false;
-            if constexpr (F::LG_EPT == 4)
-                done = warp_path && launch_warp<F>(gpu, d, tb, buf[d.src], buf[d.dst], 1u << (lg_n - d.lg_r), stream);
+            if constexpr (F::LG_EPT == 4) {
+                if (warp_path) {
+                    // the warp passes address a launch's elements in 32 bits: a batch past 2^31
+                    // elements goes in launches of whole rows, each on its own slice of the buffers
+                    const size_t rows = std::max<size_t>(1, ((size_t)1 << 31) >> lg_n);
+                    done = true;
+                    for (size_t r0 = 0; r0 < batch && done; r0 += rows) {
+                        const size_t off = r0 << lg_n, nr = std::min(rows, batch - r0);
+                        done = launch_warp<F>(gpu, d, tb, buf[d.src] + off, buf[d.dst] + off,
+                                              (uint32_t)(nr << (lg_n - d.lg_r)), stream);
+                    }
+                }
+            }
             if (!done && !launch_static<F>(d, tb, buf[d.src], buf[d.dst], ntiles, smem, stream))
                 pass_kernel<F><<<ntiles, tile_threads<F>(d), smem, stream>>>(d, tb, buf[d.src], buf[d.dst]);
             COUNT_LAUNCH();
@@ -340,7 +358,7 @@ public:
         if (scratch) CUDA_OK(cudaFreeAsync(scratch, stream));
 
         if (inverse && type == Type::coset)
-            coset_scale(gpu, d_inout, lg_n, out_rev, true, stream);
+            coset_scale(gpu, d_inout, lg_n, out_rev, true, stream, batch);
     }
 
     // one local stage of the slab-sharded transform (ntt_plan.hpp: make_slab_plan); which = 1:
@@ -478,6 +496,112 @@ public:
     static void Base_dev_ptr(const gpu_t& gpu, cudaStream_t stream, T* d_inout, uint32_t lg_n,
                              InputOutputOrder order, Direction direction, Type type)
     {   NTT_internal(gpu, d_inout, lg_n, order, direction, type, stream);   }
+
+    // rejects a batch whose byte size does not fit size_t (callers validate before any work)
+    static bool batch_fits(uint32_t lg_n, size_t batch)
+    {   return lg_n <= 30 && batch <= (SIZE_MAX / sizeof(T)) >> lg_n;   }
+
+    // batched LDE on device memory, enqueued on `stream`: d_in holds `batch` rows of 2^lg_n
+    // evaluations and is left holding each row's coefficients in bit-reversed order; d_out receives
+    // `batch` rows of 2^(lg_n + lg_blowup) evaluations on the coset, natural order (row by row what
+    // LDE returns)
+    static void LDE_batch_dev(const gpu_t& gpu, cudaStream_t stream, T* d_out, T* d_in, uint32_t lg_n,
+                              uint32_t lg_blowup, size_t batch)
+    {
+        if (lg_n > 30 || lg_blowup > 30)
+            throw cuda_error(-(int)cudaErrorInvalidValue, "LDE: lg_domain_size + lg_blowup out of range for this field");
+        const uint32_t lg_ext = lg_n + lg_blowup;
+        if (lg_ext > (uint32_t)F::MAX_LG || lg_ext > 30 || !batch_fits(lg_ext, batch))
+            throw cuda_error(-(int)cudaErrorInvalidValue, "LDE: lg_domain_size + lg_blowup out of range for this field");
+        if (lg_n == 0 || batch == 0) return;
+        // the spread reads every row of d_in while writing d_out: the two must not overlap
+        const size_t n_in = batch << lg_n, n_out = batch << lg_ext;
+        if (d_in < d_out + n_out && d_out < d_in + n_in)
+            throw cuda_error(-(int)cudaErrorInvalidValue, "LDE batch: d_out overlaps d_in");
+        NTT_internal(gpu, d_in, lg_n, InputOutputOrder::NR, Direction::inverse, Type::standard, stream, batch);
+        const CosetTables& ct = coset_tables(gpu, false, stream);
+        const size_t n_ext = batch << lg_ext;
+        uint32_t blocks = (uint32_t)std::min<size_t>((n_ext + 255) / 256, (size_t)gpu.sm_count() * 16);
+        lde_spread_kernel<F><<<blocks, 256, 0, stream>>>(d_out, d_in, lg_n, lg_blowup, ct.g0, ct.g1, ct.g2, true, batch);
+        COUNT_LAUNCH();
+        CUDA_OK(cudaGetLastError());
+        NTT_internal(gpu, d_out, lg_ext, InputOutputOrder::RN, Direction::forward, Type::standard, stream, batch);
+    }
+
+    // batched host-pointer entry: `batch` rows of 2^lg_n elements in place, synchronised.  The rows
+    // travel in groups of about GROUP_BYTES through up to three device buffers: while group g is
+    // transformed on stream 0, group g + 1 is uploaded on stream 1 and group g - 1 downloaded on
+    // stream 2 (copies overlap transforms for pinned or registered memory; pageable memory goes
+    // through the pinned staging ring, as in Base)
+    static constexpr size_t GROUP_BYTES = (size_t)32 << 20;
+    static RustError Base_batch(const gpu_t& gpu, T* inout, uint32_t lg_n, size_t batch, InputOutputOrder order,
+                                Direction direction, Type type)
+    {
+        if (lg_n > (uint32_t)F::MAX_LG || lg_n > 30 || !batch_fits(lg_n, batch))   // before touching the buffer
+            return rust_err(-(int)cudaErrorInvalidValue, "NTT batch: lg_domain_size or batch out of range for this field");
+        if (lg_n == 0 || batch == 0) return rust_ok();
+        const size_t row_bytes = sizeof(T) << lg_n;
+        const size_t rows = std::min(batch, std::max<size_t>(1, GROUP_BYTES / row_bytes));
+        // three buffers keep upload, transform and download all busy; groups of a GiB or more (one
+        // huge row) make do with two.  Two or more buffers whenever there are two or more groups:
+        // the upload of group g waits for the download of group g - nbuf, enqueued one step earlier
+        const size_t ngroups = (batch + rows - 1) / rows;
+        const size_t nbuf = std::min<size_t>(ngroups, rows * row_bytes >= ((size_t)1 << 30) ? 2 : 3);
+        T* dbuf = nullptr;
+        RustError result = rust_ok();
+        try {
+            gpu.select();
+            const stream_t &comp = gpu[0], &up = gpu[1], &down = gpu[2];
+            const bool pageable = batch * row_bytes >= ((size_t)8 << 20) && stager_t::is_pageable(inout);
+            std::unique_lock<std::mutex> stage_lock(gpu.stage_mtx, std::defer_lock);
+            if (pageable) stage_lock.lock();
+            CUDA_OK(cudaMallocAsync((void**)&dbuf, nbuf * rows * row_bytes, comp));
+            event_t allocated, uploaded[3], computed[3], downloaded[3];
+            allocated.record(comp);
+            allocated.wait(up);
+            auto group = [&](size_t g, T*& dev, T*& host, size_t& bytes) {
+                dev = dbuf + (g % nbuf) * (rows << lg_n);
+                host = inout + ((g * rows) << lg_n);
+                bytes = std::min(rows, batch - g * rows) * row_bytes;
+            };
+            // step i: upload + transform group i, then download group i - 1, so that a host-blocking
+            // (pageable) copy of one group runs while the neighbouring group is being transformed
+            for (size_t i = 0; i <= ngroups; i++) {
+                T *dev, *host;
+                size_t bytes;
+                if (i < ngroups) {
+                    group(i, dev, host, bytes);
+                    const size_t b = i % nbuf;
+                    if (i >= nbuf) downloaded[b].wait(up);        // buffer b's previous group has left
+                    if (pageable) gpu.stager().HtoD(up, dev, host, bytes);
+                    else up.HtoD(dev, host, bytes);
+                    uploaded[b].record(up);
+                    uploaded[b].wait(comp);
+                    NTT_internal(gpu, dev, lg_n, order, direction, type, comp, bytes / row_bytes);
+                    computed[b].record(comp);
+                }
+                if (i >= 1) {
+                    group(i - 1, dev, host, bytes);
+                    const size_t b = (i - 1) % nbuf;
+                    computed[b].wait(down);
+                    if (pageable) gpu.stager().DtoH(down, host, dev, bytes);
+                    else down.DtoH(host, dev, bytes);
+                    downloaded[b].record(down);
+                }
+            }
+            downloaded[(ngroups - 1) % nbuf].wait(comp);
+            CUDA_OK(cudaFreeAsync(dbuf, comp));
+            dbuf = nullptr;
+            gpu.sync();
+        } catch (const cuda_error& e) {
+            result = rust_err(e.code(), e.what());
+        }
+        if (dbuf) {
+            try { gpu.sync(); } catch (...) {}
+            (void)cudaFreeAsync(dbuf, gpu[0]);
+        }
+        return result;
+    }
 
     // host-pointer entry: alloc + HtoD + transform + DtoH + sync, errors -> RustError
     static RustError Base(const gpu_t& gpu, T* inout, uint32_t lg_n, InputOutputOrder order,

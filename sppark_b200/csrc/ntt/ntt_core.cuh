@@ -58,6 +58,20 @@ struct Pass {
     uint64_t peer[8];
 };
 
+// coset factor of element i of a batch of 2^lg_n-point transforms: g^e, e = the element's
+// position within its transform, bit-reversed if `bitrev`; g0/g1/g2 hold g^i, g^(i << 12),
+// g^(i << 24)
+template<class F>
+HD typename F::T coset_mul(typename F::T x, uint64_t i, uint32_t lg_n, bool bitrev,
+                           const typename F::T* g0, const typename F::T* g1, const typename F::T* g2)
+{
+    const uint32_t j = (uint32_t)i & ((1u << lg_n) - 1), e = bitrev ? brev32(j, lg_n) : j;
+    x = F::mul(x, g0[e & 4095]);
+    if (e >> 12) x = F::mul(x, g1[(e >> 12) & 4095]);
+    if (e >> 24) x = F::mul(x, g2[e >> 24]);
+    return x;
+}
+
 template<class F> struct Tables {
     const typename F::T* dense;          // dense[h + i] = w_(2h)^i, h = 1,2,4..2^(LG_DENSE-1)
     const typename F::T* tlo;            // tlo[i] = w_N^i,            i < 2^LG_TLO

@@ -147,6 +147,29 @@ inline Plan make_plan(uint32_t lg_n, int order, bool inverse, uint32_t lg_tile,
     return plan;
 }
 
+// Turns a plan of make_plan into the same transform over `batch` rows of 2^lg_n elements stored one
+// after another in every buffer the passes touch (scratch included).  The row index becomes the
+// most significant digit of the tile index: a pass then has batch x its single-transform tile count,
+// tile t is tile t mod 2^lg_tpt (lg_tpt = lg_n - lg_r - lg_w) of row t >> lg_tpt.  In the
+// descriptor's address term th * (t >> lg_tlo) this is free: a tile layout with a high term already
+// has th << (lg_tpt - lg_tlo) == 2^lg_n (the high term is the top index digit), one without
+// (lg_tlo = 32) gets lg_tlo = lg_tpt, th = 2^lg_n.  Twiddle columns read bits below lg_n only
+// (tw_rsh + tw_bits <= lg_n), so they see the in-row position.  No kernel changes, and batch 1
+// leaves the descriptor as it is.  Slab and peer passes route rows elsewhere and cannot be batched:
+// returns false for them.
+inline bool set_batch(Plan& plan, uint64_t batch)
+{
+    for (Pass& d : plan.passes)
+        if (d.out_split_bits || d.peer_on || d.tw_col_offset) return false;
+    if (batch <= 1) return true;
+    for (Pass& d : plan.passes) {
+        const uint32_t lg_tpt = plan.lg_n - d.lg_r - d.lg_w;
+        if (d.in_lg_tlo >= 32) { d.in_lg_tlo = lg_tpt; d.in_th = 1ull << plan.lg_n; }
+        if (d.out_lg_tlo >= 32) { d.out_lg_tlo = lg_tpt; d.out_th = 1ull << plan.lg_n; }
+    }
+    return true;
+}
+
 // ---- slab-sharded transform over G = 2^lg_g ranks, ONE all-to-all ---------------------------
 // N = N1 x N2 (N1 = 2^s1 rows, N2 = 2^s2 columns, x[j1*N2 + j2]).  Rank r owns the columns
 // j2 in [r*N2/G, (r+1)*N2/G) of the input, stored locally as a row-major [N1][N2/G] matrix, and

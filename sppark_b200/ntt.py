@@ -91,3 +91,69 @@ def ntt_dev(tensor, order=NN, direction=FORWARD, typ=STANDARD, field=None, strea
         err = _lib.lib().sppark_b200_ntt_dev(field, tensor.data_ptr(), n.bit_length() - 1,
                                              order, direction, typ, s)
     _lib.check(err)
+
+
+def _batch_shape(shape, itemsize, field):
+    """(batch, n) for the one-word fields, (batch, n, 4) uint64 words for the 256-bit fields; the
+    element size must be the field's word size, or the library would run past the buffer"""
+    wide = field not in (GL64, BB31)
+    if itemsize != (4 if field == BB31 else 8):
+        raise ValueError(f"{itemsize}-byte elements do not match field {field}")
+    if len(shape) != (3 if wide else 2) or (wide and shape[2] != 4):
+        raise ValueError("batched arrays are (batch, n)" + (", 4) uint64 for this field" if wide else ""))
+    batch, n = int(shape[0]), int(shape[1])
+    if n == 0 or n & (n - 1):
+        raise ValueError("row length is not a power of 2")
+    return batch, n.bit_length() - 1
+
+
+def ntt_batch(device_id, inout, order=NN, direction=FORWARD, typ=STANDARD, field=None):
+    """`batch` same-size transforms in one call, in place on a host array: row b of a C-contiguous
+    (batch, n) array (or (batch, n, 4) uint64 for the 256-bit fields) comes out as
+    NTT/iNTT/coset_* would return it alone.  Synchronised."""
+    if not isinstance(inout, np.ndarray) or not inout.flags["C_CONTIGUOUS"] or not inout.flags["WRITEABLE"]:
+        raise TypeError("inout must be a writable C-contiguous numpy array")
+    field = _field_of(inout) if field is None else field
+    batch, lg = _batch_shape(inout.shape, inout.itemsize, field)
+    _lib.check(_lib.lib().sppark_b200_ntt_batch(field, device_id, inout.ctypes.data, lg, batch,
+                                                order, direction, typ))
+
+
+def _dev_field(tensor, field):
+    if field is None:
+        if tensor.element_size() not in (4, 8):
+            raise ValueError("tensor elements must be 8 bytes (Goldilocks) or 4 bytes (BabyBear)")
+        field = {8: GL64, 4: BB31}[tensor.element_size()]
+    return field
+
+
+def ntt_batch_dev(tensor, order=NN, direction=FORWARD, typ=STANDARD, field=None, stream=None):
+    """ntt_batch on a CUDA torch tensor of the same shapes: in place, enqueued on torch's current
+    stream (or `stream`), not synchronised."""
+    import torch
+    if not tensor.is_cuda or not tensor.is_contiguous():
+        raise ValueError("tensor must be a contiguous CUDA tensor")
+    field = _dev_field(tensor, field)
+    batch, lg = _batch_shape(tuple(tensor.shape), tensor.element_size(), field)
+    with torch.cuda.device(tensor.device):
+        s = stream if stream is not None else torch.cuda.current_stream().cuda_stream
+        err = _lib.lib().sppark_b200_ntt_batch_dev(field, tensor.data_ptr(), lg, batch, order, direction, typ, s)
+    _lib.check(err)
+
+
+def lde_batch_dev(d_in, lg_blowup, field=None, stream=None):
+    """LDE of every row of a (batch, n) CUDA tensor (or (batch, n, 4) for the 256-bit fields):
+    returns a new (batch, n << lg_blowup) tensor whose rows are what LDE returns for each row,
+    and leaves each row's coefficients, in bit-reversed order, in d_in.  Enqueued on torch's
+    current stream (or `stream`), not synchronised."""
+    import torch
+    if not d_in.is_cuda or not d_in.is_contiguous():
+        raise ValueError("d_in must be a contiguous CUDA tensor")
+    field = _dev_field(d_in, field)
+    batch, lg = _batch_shape(tuple(d_in.shape), d_in.element_size(), field)
+    out = torch.empty((batch, (1 << lg) << lg_blowup) + tuple(d_in.shape[2:]), dtype=d_in.dtype, device=d_in.device)
+    with torch.cuda.device(d_in.device):
+        s = stream if stream is not None else torch.cuda.current_stream().cuda_stream
+        err = _lib.lib().sppark_b200_lde_batch_dev(field, out.data_ptr(), d_in.data_ptr(), lg, lg_blowup, batch, s)
+    _lib.check(err)
+    return out
