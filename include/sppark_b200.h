@@ -266,6 +266,13 @@ RustError sppark_b200_selftest_field(int field, int op, size_t n, void *r, const
  * Montgomery words): op 0 mul (Goldilocks: b is a canonical constant in Montgomery form, the result
  * a*b*2^-64 mod p, see csrc/ff/gl64.cuh), 1 add, 2 sub (b canonical), 3 tight, 4 canon. */
 RustError sppark_b200_selftest_word_field(int field, int op, size_t n, void *r, const void *a, const void *b);
+/* device self-test hook for the MSM's bucket sort: n host scalars (8 little-endian 32-bit words
+ * each), window width wbits (3..24), cap entries per bin-sort CTA (0 = default; smaller values
+ * send more bins down the overflow path).  Host outputs: counts and offsets per (window, bucket)
+ * slot (nwins << (wbits - 1) each), the sorted entries (nwins * n), one slot per heavy bucket, and
+ * info = {nwins, heavy threshold, #heavy buckets, log2 bins per window, #overflow bins}. */
+RustError sppark_b200_selftest_msm_sort(size_t n, uint32_t wbits, uint32_t cap, const void *scalars, void *counts,
+                                        void *offsets, void *sorted, void *heavy_slots, uint32_t *info);
 
 /* introspection */
 size_t      sppark_b200_ngpus(void);               /* ngpus(), util/gpu_t.cuh:21 */

@@ -57,6 +57,8 @@ _SIGS = {
     "sppark_b200_msm_sharded": [C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t],
     "sppark_b200_ntt_sharded": [C.c_int, C.c_void_p, C.c_uint32, C.c_int, C.c_void_p, C.c_size_t],
     "sppark_b200_selftest_word_field": [C.c_int, C.c_int, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p],
+    "sppark_b200_selftest_msm_sort": [C.c_size_t, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_void_p, C.c_void_p],
     "sppark_b200_prefix_op_dev": [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p],
     "sppark_b200_div_by_x_minus_z_dev": [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int, C.c_void_p],
     "sppark_b200_evaluate_dev": [C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p],

@@ -16,80 +16,260 @@ namespace msm {
 constexpr uint32_t ACC_THREADS = SPPARK_B200_ACC_THREADS;       // accumulate CTA size
 constexpr uint32_t HEAVY_THREADS = 128;
 
-static __global__ void count_kernel(const Config cfg, const uint32_t* scalars, uint32_t* counts)
-{
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < cfg.npoints; i += gridDim.x * blockDim.x)
-        count_body(cfg, scalars, counts, i);
-}
+// ---- sort (msm_core.cuh, "sort"): bin histogram -> bin scan -> partition -> bin sort -> overflow ----
+constexpr uint32_t HIST_THREADS = 1024;
+constexpr uint32_t HIST_SMEM_WORDS = 56 * 1024;     // bin counters of one histogram CTA (224 KB)
+constexpr uint32_t SORT_THREADS = 512;
+// entries one bin-sort CTA places through shared memory: with the 2^SORT_SMAX bucket cursors 112 KB,
+// two CTAs per SM.  Uniform windows fill a bin to ~2^13 entries at any size up to 2^28 points; the
+// top window of 254-bit scalars fills its used bins to ~2^14.
+constexpr uint32_t SORT_CAP = 24576;
 
-
-// control block: [0] task counter, [1] #heavy buckets, [2] #chunks
-// heavy bucket h: heavy_list[3h] = slot, [3h+1] = first chunk, [3h+2] = #chunks; chunk_map[c] = h
-// one CTA (1024 threads) per window: exclusive prefix of the bucket histogram in tiles of 4096
-// counters (one 128-bit load per thread, warp-shuffle scans); heavy buckets get chunked
-static __global__ void __launch_bounds__(1024)
-scan_kernel(const Config cfg, const uint32_t* counts, uint32_t* offsets, uint32_t* cursor,
-            uint32_t* ctrl, uint32_t* heavy_list, uint32_t* chunk_map)
+// exclusive prefix over len values (four consecutive per thread, tiles of 4 * blockDim);
+// visit(j, value_j, prefix_j) for every j < len, returns the total.  Every thread of the CTA calls it.
+template<class Load, class Visit>
+__device__ uint32_t block_exclusive_scan(uint32_t len, Load load, Visit visit)
 {
     __shared__ uint32_t warp_tot[32];
-    const uint32_t w = blockIdx.x, nb = 1u << cfg.lg_nb;            // nb >= 8: a multiple of 4
-    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const size_t base = (size_t)w << cfg.lg_nb;
+    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
     uint32_t carry = 0;                                             // total of the tiles before this one
-    for (uint32_t t0 = 0; t0 < nb; t0 += 4096) {
-        const uint32_t b = t0 + threadIdx.x * 4;
-        uint4 c = make_uint4(0, 0, 0, 0);
-        if (b < nb) c = *reinterpret_cast<const uint4*>(counts + base + b);
-        const uint32_t s = c.x + c.y + c.z + c.w;
+    for (uint32_t t0 = 0; t0 < len; t0 += 4 * blockDim.x) {
+        const uint32_t b = t0 + 4 * threadIdx.x;
+        uint32_t c[4];
+#pragma unroll
+        for (uint32_t k = 0; k < 4; k++) c[k] = b + k < len ? load(b + k) : 0;
+        const uint32_t s = c[0] + c[1] + c[2] + c[3];
         uint32_t x = s;                                             // inclusive scan inside the warp
 #pragma unroll
         for (uint32_t d = 1; d < 32; d <<= 1) {
-            uint32_t y = __shfl_up_sync(0xffffffffu, x, d);
+            const uint32_t y = __shfl_up_sync(0xffffffffu, x, d);
             if (lane >= d) x += y;
         }
         if (lane == 31) warp_tot[wid] = x;
         __syncthreads();
         if (wid == 0) {
-            uint32_t t = warp_tot[lane];
+            uint32_t t = lane < nw ? warp_tot[lane] : 0;
 #pragma unroll
             for (uint32_t d = 1; d < 32; d <<= 1) {
-                uint32_t y = __shfl_up_sync(0xffffffffu, t, d);
+                const uint32_t y = __shfl_up_sync(0xffffffffu, t, d);
                 if (lane >= d) t += y;
             }
             warp_tot[lane] = t;
         }
         __syncthreads();
-        uint4 r;
-        r.x = carry + (wid ? warp_tot[wid - 1] : 0) + x - s;
-        r.y = r.x + c.x;
-        r.z = r.y + c.y;
-        r.w = r.z + c.z;
+        uint32_t r = carry + (wid ? warp_tot[wid - 1] : 0) + x - s;
         carry += warp_tot[31];
-        if (b < nb) {
-            *reinterpret_cast<uint4*>(offsets + base + b) = r;
-            *reinterpret_cast<uint4*>(cursor + base + b) = r;
-            const uint32_t cc[4] = {c.x, c.y, c.z, c.w};
 #pragma unroll
-            for (uint32_t k = 0; k < 4; k++) {
-                if (cc[k] > cfg.heavy) {
-                    uint32_t h = atomicAdd(&ctrl[1], 1), nch = (cc[k] + cfg.heavy_chunk - 1) / cfg.heavy_chunk;
-                    uint32_t first_chunk = atomicAdd(&ctrl[2], nch);
-                    heavy_list[3 * h] = (uint32_t)(base + b + k);
-                    heavy_list[3 * h + 1] = first_chunk;
-                    heavy_list[3 * h + 2] = nch;
-                    for (uint32_t q = 0; q < nch; q++) chunk_map[first_chunk + q] = h;
-                }
-            }
+        for (uint32_t k = 0; k < 4; k++) {
+            if (b + k < len) visit(b + k, c[k], r);
+            r += c[k];
         }
         __syncthreads();                                            // warp_tot is reused by the next tile
     }
+    return carry;
 }
 
-static __global__ void scatter_kernel(const Config cfg, const uint32_t* scalars, uint32_t* cursor, uint32_t* sorted,
-                                      uint32_t w0, uint32_t w1)
+// pass 1: bin histogram of the windows [w0, w0 + wpg) of group blockIdx.y in shared memory, one
+// global atomic per non-zero counter per CTA; a warp adds equal bins once (all scalars equal:
+// every lane of the warp hits one counter)
+static __global__ void __launch_bounds__(HIST_THREADS)
+bin_hist_kernel(const Config cfg, uint32_t lg_bins, const uint32_t* scalars, uint32_t wpg, uint32_t* bin_count)
 {
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < cfg.npoints; i += gridDim.x * blockDim.x)
-        scatter_body(cfg, scalars, cursor, sorted, i, w0, w1);
+    extern __shared__ uint32_t hist[];
+    const uint32_t w0 = blockIdx.y * wpg, w1 = min(w0 + wpg, cfg.nwins), nctr = (w1 - w0) << lg_bins;
+    const uint32_t lane = threadIdx.x & 31;
+    for (uint32_t k = threadIdx.x; k < nctr; k += blockDim.x) hist[k] = 0;
+    __syncthreads();
+    for (uint32_t i0 = blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < cfg.npoints; i0 += gridDim.x * blockDim.x) {
+        const uint32_t i = i0 + lane;                               // whole warps iterate together
+        for_each_digit(cfg, lg_bins, scalars, i, i < cfg.npoints, w1,
+                       [&](uint32_t w, bool nz, uint32_t bin, uint32_t, uint32_t) {
+            if (w < w0) return;                                     // the same for the whole warp
+            const uint32_t key = nz ? bin - (w0 << lg_bins) : ~0u;
+            const uint32_t peers = __match_any_sync(0xffffffffu, key);
+            if (nz && lane == __ffs(peers) - 1) atomicAdd(&hist[key], __popc(peers));
+        });
+    }
+    __syncthreads();
+    for (uint32_t k = threadIdx.x; k < nctr; k += blockDim.x)
+        if (hist[k]) atomicAdd(&bin_count[((size_t)w0 << lg_bins) + k], hist[k]);
+}
+
+// one CTA per window: window-local bin bases, and the partition's cursors
+static __global__ void __launch_bounds__(1024)
+bin_scan_kernel(uint32_t lg_bins, const uint32_t* bin_count, uint32_t* bin_base, uint32_t* bin_cur)
+{
+    const size_t row = (size_t)blockIdx.x << lg_bins;
+    block_exclusive_scan(1u << lg_bins, [&](uint32_t j) { return bin_count[row + j]; },
+                         [&](uint32_t j, uint32_t, uint32_t off) { bin_base[row + j] = off; bin_cur[row + j] = off; });
+}
+
+// pass 2: every (point, window) entry appended at its bin's cursor, one reservation per distinct
+// bin per warp.  All windows in one pass: the open frontier is one partly written line per bin
+// (W * 2^lg_bins * 128 B, 13.6 MB at 2^26 points), so lines fill in L2 and leave whole.
+static __global__ void __launch_bounds__(256)
+partition_kernel(const Config cfg, uint32_t lg_bins, const uint32_t* scalars, uint32_t* bin_cur, uint2* staging)
+{
+    const uint32_t lane = threadIdx.x & 31;
+    for (uint32_t i0 = blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < cfg.npoints; i0 += gridDim.x * blockDim.x) {
+        const uint32_t i = i0 + lane;
+        for_each_digit(cfg, lg_bins, scalars, i, i < cfg.npoints, cfg.nwins,
+                       [&](uint32_t w, bool nz, uint32_t bin, uint32_t b, uint32_t entry) {
+            const uint32_t peers = __match_any_sync(0xffffffffu, nz ? bin : ~0u);
+            const uint32_t leader = __ffs(peers) - 1;
+            uint32_t pos = 0;
+            if (nz && lane == leader) pos = atomicAdd(&bin_cur[bin], __popc(peers));
+            pos = __shfl_sync(0xffffffffu, pos, leader) + __popc(peers & ((1u << lane) - 1));
+            if (nz) staging[(size_t)w * cfg.npoints + pos] = make_uint2(entry, b);
+        });
+    }
+}
+
+// pass 3: one CTA per bin (blockIdx.x = w << lg_bins | bin).  Bucket histogram of the bin in
+// shared memory, counts / offsets / heavy buckets for its buckets, the entries placed into a
+// shared copy of the bin's output range, which is then written out coalesced.  A bin of more than
+// `cap` entries is listed for the overflow path instead.
+static __global__ void __launch_bounds__(SORT_THREADS)
+bin_sort_kernel(const Config cfg, uint32_t lg_bins, uint32_t cap, const uint2* staging, const uint32_t* bin_count,
+                const uint32_t* bin_base, uint32_t* counts, uint32_t* offsets, uint32_t* sorted, uint32_t* ctrl,
+                uint32_t* heavy_list, uint32_t* chunk_map, uint32_t* overflow)
+{
+    extern __shared__ uint32_t sm[];                        // [cap] output run, [2^SORT_SMAX] bucket cursors
+    const uint32_t w = blockIdx.x >> lg_bins, bin = blockIdx.x & ((1u << lg_bins) - 1);
+    uint32_t b0, nbk;
+    if (!bin_buckets(cfg, lg_bins, w, bin, b0, nbk)) return;
+    const uint32_t cnt = bin_count[blockIdx.x], base = bin_base[blockIdx.x];
+    const size_t t0 = ((size_t)w << cfg.lg_nb) + b0;
+    if (last_bin(cfg, lg_bins, w, bin))                     // buckets no digit reaches (top window)
+        for (uint32_t b = b0 + nbk + threadIdx.x; b < (1u << cfg.lg_nb); b += blockDim.x)
+            offsets[((size_t)w << cfg.lg_nb) + b] = base + cnt;
+    if (cnt > cap) {
+        if (threadIdx.x == 0) overflow[atomicAdd(&ctrl[3], 1)] = blockIdx.x;
+        return;
+    }
+    uint32_t *run = sm, *cur = sm + cap;
+    for (uint32_t k = threadIdx.x; k < nbk; k += blockDim.x) cur[k] = 0;
+    __syncthreads();
+    const uint2* src = staging + (size_t)w * cfg.npoints + base;
+    for (uint32_t k = threadIdx.x; k < cnt; k += blockDim.x) atomicAdd(&cur[src[k].y - b0], 1);
+    __syncthreads();
+    block_exclusive_scan(nbk, [&](uint32_t j) { return cur[j]; }, [&](uint32_t j, uint32_t c, uint32_t off) {
+        counts[t0 + j] = c;
+        offsets[t0 + j] = base + off;
+        cur[j] = off;
+        register_heavy(cfg, (uint32_t)(t0 + j), c, ctrl, heavy_list, chunk_map);
+    });
+    for (uint32_t k = threadIdx.x; k < cnt; k += blockDim.x) {
+        const uint2 e = src[k];
+        run[atomicAdd(&cur[e.y - b0], 1)] = e.x;
+    }
+    __syncthreads();
+    uint32_t* dst = sorted + (size_t)w * cfg.npoints + base;
+    for (uint32_t k = threadIdx.x; k < cnt; k += blockDim.x) dst[k] = run[k];
+}
+
+// overflow path, over the entries of every listed bin in turn (grid-stride): PLACE = false adds
+// them to `slots` = counts, PLACE = true places them at `slots` = cursor.  One global atomic per
+// distinct bucket per warp: a bucket holding every point costs n / 32 atomics.
+template<bool PLACE>
+__global__ void __launch_bounds__(256)
+overflow_kernel(const Config cfg, uint32_t lg_bins, const uint2* staging, const uint32_t* bin_count,
+                const uint32_t* bin_base, const uint32_t* ctrl, const uint32_t* overflow, uint32_t* slots,
+                uint32_t* sorted)
+{
+    const uint32_t lane = threadIdx.x & 31, nov = ctrl[3];
+    for (uint32_t o = 0; o < nov; o++) {
+        const uint32_t g = overflow[o], w = g >> lg_bins, cnt = bin_count[g];
+        const uint2* src = staging + (size_t)w * cfg.npoints + bin_base[g];
+        uint32_t* row = slots + ((size_t)w << cfg.lg_nb);
+        for (uint32_t k0 = blockIdx.x * blockDim.x + (threadIdx.x & ~31u); k0 < cnt; k0 += gridDim.x * blockDim.x) {
+            const uint32_t k = k0 + lane;
+            const uint2 e = k < cnt ? src[k] : make_uint2(0, ~0u);
+            const uint32_t peers = __match_any_sync(0xffffffffu, e.y);
+            const uint32_t leader = __ffs(peers) - 1;
+            uint32_t pos = 0;
+            if (k < cnt && lane == leader) pos = atomicAdd(&row[e.y], __popc(peers));
+            if (PLACE) {
+                pos = __shfl_sync(0xffffffffu, pos, leader) + __popc(peers & ((1u << lane) - 1));
+                if (k < cnt) sorted[(size_t)w * cfg.npoints + pos] = e.x;
+            }
+        }
+    }
+}
+
+// overflow path, between the two passes: one CTA per listed bin, offsets / cursors / heavy buckets
+static __global__ void __launch_bounds__(1024)
+overflow_scan_kernel(const Config cfg, uint32_t lg_bins, const uint32_t* bin_base, const uint32_t* overflow,
+                     const uint32_t* counts, uint32_t* offsets, uint32_t* cursor, uint32_t* ctrl,
+                     uint32_t* heavy_list, uint32_t* chunk_map)
+{
+    const uint32_t nov = ctrl[3];
+    for (uint32_t o = blockIdx.x; o < nov; o += gridDim.x) {
+        const uint32_t g = overflow[o], w = g >> lg_bins, base = bin_base[g];
+        uint32_t b0, nbk;
+        bin_buckets(cfg, lg_bins, w, g & ((1u << lg_bins) - 1), b0, nbk);
+        const size_t t0 = ((size_t)w << cfg.lg_nb) + b0;
+        block_exclusive_scan(nbk, [&](uint32_t j) { return counts[t0 + j]; }, [&](uint32_t j, uint32_t c, uint32_t off) {
+            offsets[t0 + j] = base + off;
+            cursor[t0 + j] = base + off;
+            register_heavy(cfg, (uint32_t)(t0 + j), c, ctrl, heavy_list, chunk_map);
+        });
+    }
+}
+
+// device buffers of the sort; nbins = nwins << sort_lg_bins(cfg, slice capacity).
+// control block ctrl: [0] accumulate's task counter, [1] #heavy buckets, [2] #chunks, [3] #overflow bins
+struct SortBufs {
+    uint32_t *counts, *offsets, *cursor, *ctrl, *heavy_list, *chunk_map, *sorted;
+    uint32_t *bin_count, *bin_base, *bin_cur, *overflow;
+    uint2* staging;                 // nwins * slice capacity entries
+};
+
+// finer profile marks inside the sort (tools/probe_msm_sort.py); off by default, so that the
+// "sort" phase stays one number
+inline bool sort_profile() { const char* e = getenv("SPPARK_B200_MSM_SORT_PROFILE"); return e && atoi(e) != 0; }
+
+// (window, bucket) lists of cfg.npoints scalars: counts, offsets, sorted, ctrl[1..3], heavy_list,
+// chunk_map.  cap <= SORT_CAP: entries per bin-sort CTA (smaller values send more bins down the
+// overflow path; the self-test uses that).
+inline void sort_slice(const Config& cfg, uint32_t cap, const uint32_t* d_scalars, const SortBufs& s, uint32_t sms,
+                       cudaStream_t stream)
+{
+    const uint32_t lg_bins = sort_lg_bins(cfg, cfg.npoints);
+    const size_t nbins = (size_t)cfg.nwins << lg_bins, nslots = (size_t)cfg.nwins << cfg.lg_nb;
+    const bool marks = sort_profile();
+    CUDA_OK(cudaFuncSetAttribute(bin_hist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, HIST_SMEM_WORDS * 4));
+    CUDA_OK(cudaFuncSetAttribute(bin_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (SORT_CAP + (1u << SORT_SMAX)) * 4));
+    CUDA_OK(cudaMemsetAsync(s.counts, 0, nslots * 4, stream));
+    CUDA_OK(cudaMemsetAsync(s.ctrl, 0, 16, stream));
+    CUDA_OK(cudaMemsetAsync(s.bin_count, 0, nbins * 4, stream));
+    const uint32_t wpg = std::min(cfg.nwins, HIST_SMEM_WORDS >> lg_bins);
+    const uint32_t ngroups = (cfg.nwins + wpg - 1) / wpg;
+    const uint32_t hist_blk = (uint32_t)std::min<size_t>((cfg.npoints + HIST_THREADS - 1) / HIST_THREADS, sms);
+    bin_hist_kernel<<<dim3(hist_blk, ngroups), HIST_THREADS, ((size_t)wpg << lg_bins) * 4, stream>>>(
+        cfg, lg_bins, d_scalars, wpg, s.bin_count);
+    COUNT_LAUNCH();
+    bin_scan_kernel<<<cfg.nwins, 1024, 0, stream>>>(lg_bins, s.bin_count, s.bin_base, s.bin_cur);
+    COUNT_LAUNCH();
+    if (marks) g_profile.mark("sort_partition", stream);
+    const uint32_t part_blk = (uint32_t)std::min<size_t>((cfg.npoints + 255) / 256, (size_t)sms * 8);
+    partition_kernel<<<part_blk, 256, 0, stream>>>(cfg, lg_bins, d_scalars, s.bin_cur, s.staging);
+    COUNT_LAUNCH();
+    if (marks) g_profile.mark("sort_bins", stream);
+    bin_sort_kernel<<<(uint32_t)nbins, SORT_THREADS, (cap + (1u << SORT_SMAX)) * 4, stream>>>(
+        cfg, lg_bins, cap, s.staging, s.bin_count, s.bin_base, s.counts, s.offsets, s.sorted, s.ctrl,
+        s.heavy_list, s.chunk_map, s.overflow);
+    COUNT_LAUNCH();
+    if (marks) g_profile.mark("sort_overflow", stream);
+    overflow_kernel<false><<<sms * 4, 256, 0, stream>>>(cfg, lg_bins, s.staging, s.bin_count, s.bin_base, s.ctrl,
+                                                        s.overflow, s.counts, s.sorted);
+    overflow_scan_kernel<<<sms, 1024, 0, stream>>>(cfg, lg_bins, s.bin_base, s.overflow, s.counts, s.offsets, s.cursor,
+                                                   s.ctrl, s.heavy_list, s.chunk_map);
+    overflow_kernel<true><<<sms * 4, 256, 0, stream>>>(cfg, lg_bins, s.staging, s.bin_count, s.bin_base, s.ctrl,
+                                                       s.overflow, s.cursor, s.sorted);
+    COUNT_LAUNCH(); COUNT_LAUNCH(); COUNT_LAUNCH();
+    CUDA_OK(cudaGetLastError());
 }
 
 // ---- batched-affine pre-reduction of the bucket lists (msm_pair.cuh) ---------------------------
@@ -486,6 +666,8 @@ public:
         uint32_t lg_l, items1;
         uint8_t* blob;
         uint32_t *counts, *offsets, *cursor, *ctrl, *heavy_list, *chunk_map, *partials, *sorted, *buckets;
+        uint32_t *bin_count, *bin_base, *bin_cur, *overflow;
+        uint2* staging;             // the sort's bins: nwins * slice_cap entries of 8 bytes
         uint32_t *R[2], *S[2];
         uint32_t slices_done;
         // batched-affine pre-reduction (msm_pair.cuh), off unless SPPARK_B200_MSM_PAIR=1
@@ -522,6 +704,9 @@ public:
         size_t off = 0;
         auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
         const size_t o_counts = take(j.nslots * 4), o_offsets = take(j.nslots * 4), o_cursor = take(j.nslots * 4);
+        const size_t nbins = (size_t)j.cfg.nwins << sort_lg_bins(j.cfg, slice_cap);
+        const size_t o_bcount = take(nbins * 4), o_bbase = take(nbins * 4), o_bcur = take(nbins * 4), o_over = take(nbins * 4);
+        const size_t o_staging = take(entries * 8);
         const size_t o_ctrl = take(16), o_heavy = take(heavy_cap * 12), o_cmap = take(chunk_cap * 4);
         const size_t o_partials = take(chunk_cap * BW * 4);
         const size_t o_sorted = take(entries * 4);
@@ -548,6 +733,8 @@ public:
         j.counts = U32(o_counts); j.offsets = U32(o_offsets); j.cursor = U32(o_cursor);
         j.ctrl = U32(o_ctrl); j.heavy_list = U32(o_heavy); j.chunk_map = U32(o_cmap);
         j.partials = U32(o_partials); j.sorted = U32(o_sorted); j.buckets = U32(o_buckets);
+        j.bin_count = U32(o_bcount); j.bin_base = U32(o_bbase); j.bin_cur = U32(o_bcur); j.overflow = U32(o_over);
+        j.staging = reinterpret_cast<uint2*>(j.blob + o_staging);
         j.R[0] = U32(o_r0); j.S[0] = U32(o_s0); j.R[1] = U32(o_r1); j.S[1] = U32(o_s1);
         j.counts1 = U32(o_c1); j.off1 = U32(o_o1); j.wintotal = U32(o_wt); j.winbase = U32(o_wb);
         j.sums = U32(o_sums); j.pre = U32(o_pre); j.totals = U32(o_tot);
@@ -564,30 +751,9 @@ public:
         cfg.merge = j.slices_done ? 1 : 0;
         const uint32_t sms = (uint32_t)gpu.sm_count();
         g_profile.mark("sort", stream);
-        CUDA_OK(cudaMemsetAsync(j.counts, 0, j.nslots * 4, stream));
-        CUDA_OK(cudaMemsetAsync(j.ctrl, 0, 16, stream));
-        const uint32_t nblk = (uint32_t)std::min<size_t>((n + 255) / 256, (size_t)sms * 16);
-        count_kernel<<<nblk, 256, 0, stream>>>(cfg, d_scalars, j.counts);
-        COUNT_LAUNCH();
-        scan_kernel<<<cfg.nwins, 1024, 0, stream>>>(cfg, j.counts, j.offsets, j.cursor, j.ctrl, j.heavy_list, j.chunk_map);
-        COUNT_LAUNCH();
-        // The scatter writes 4 random bytes per (point, window): with all windows in flight the
-        // write set (4*n bytes per window) thrashes L2 and every store costs a 32-byte sector
-        // read + write-back in DRAM.  One launch per window confines the write set to one window's
-        // slots (4*n bytes, resident in the 50 MB L2 of an H100 up to n = 2^23) at the price of
-        // re-reading the scalars per window.
-        bool per_window = n >= (1u << 18);
-        if (const char* env = getenv("SPPARK_B200_MSM_SCATTER")) per_window = atoi(env) != 0;
-        if (per_window) {
-            for (uint32_t w = 0; w < cfg.nwins; w++) {
-                scatter_kernel<<<nblk, 256, 0, stream>>>(cfg, d_scalars, j.cursor, j.sorted, w, w + 1);
-                COUNT_LAUNCH();
-            }
-        } else {
-            scatter_kernel<<<nblk, 256, 0, stream>>>(cfg, d_scalars, j.cursor, j.sorted, 0, cfg.nwins);
-            COUNT_LAUNCH();
-        }
-        CUDA_OK(cudaGetLastError());
+        const SortBufs sb{j.counts, j.offsets, j.cursor, j.ctrl, j.heavy_list, j.chunk_map, j.sorted,
+                          j.bin_count, j.bin_base, j.bin_cur, j.overflow, j.staging};
+        sort_slice(cfg, SORT_CAP, d_scalars, sb, sms, stream);
 
         g_profile.mark("accumulate", stream);
         int occ = 1;

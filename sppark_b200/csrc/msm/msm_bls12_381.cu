@@ -86,3 +86,50 @@ RustError msm_resident_bls12_381(void* out, const void* d_points, size_t npoints
     return msm_host<ff::bls12_381_fp_t>(out, nullptr, npoints, scalars, 0, false, mont ? scalars_from_mont<ff::bls12_381_fr_t> : nullptr,
                       (const uint32_t*)d_points);
 }
+
+// ---- device self-test hook: the MSM's bucket sort alone (tests/test_msm_sort.py) -------------------
+// Host scalars (n x 8 words); window width wbits, heavy threshold as make_config(n); cap entries per
+// bin-sort CTA (0 = the default).  Host outputs: counts / offsets (nwins << (wbits-1)), sorted
+// (nwins * n), heavy_slots (one slot per heavy bucket), info = {nwins, heavy threshold, #heavy,
+// lg_bins, #overflow bins}.
+extern "C" RustError sppark_b200_selftest_msm_sort(size_t n, uint32_t wbits, uint32_t cap, const void* scalars,
+                                                   void* counts, void* offsets, void* sorted, void* heavy_slots,
+                                                   uint32_t* info)
+{
+    using namespace msm;
+    if (n == 0 || n >= (1ull << 31) || wbits < 3 || wbits > 24 || cap > SORT_CAP)
+        return rust_err(-(int)cudaErrorInvalidValue, "selftest_msm_sort: bad arguments");
+    try {
+        const gpu_t& gpu = select_gpu(-1);
+        const stream_t& s = gpu[0];
+        Config cfg = make_config(n);
+        cfg.wbits = wbits;
+        cfg.nwins = (256 + wbits - 1) / wbits;
+        cfg.lg_nb = wbits - 1;
+        const size_t nslots = (size_t)cfg.nwins << cfg.lg_nb, entries = (size_t)cfg.nwins * n;
+        const size_t nbins = (size_t)cfg.nwins << sort_lg_bins(cfg, n);
+        const size_t heavy_cap = entries / (cfg.heavy + 1) + 1, chunk_cap = entries / cfg.heavy_chunk + heavy_cap;
+        dev_ptr_t<uint32_t> d_sc(8 * n, s), d_counts(nslots, s), d_offsets(nslots, s), d_cursor(nslots, s);
+        dev_ptr_t<uint32_t> d_ctrl(4, s), d_heavy(3 * heavy_cap, s), d_cmap(chunk_cap, s), d_sorted(entries, s);
+        dev_ptr_t<uint32_t> d_bcount(nbins, s), d_bbase(nbins, s), d_bcur(nbins, s), d_over(nbins, s);
+        dev_ptr_t<uint32_t> d_staging(2 * entries, s);
+        s.HtoD(d_sc, scalars, 32 * n);
+        const SortBufs sb{d_counts, d_offsets, d_cursor, d_ctrl, d_heavy, d_cmap, d_sorted,
+                          d_bcount, d_bbase, d_bcur, d_over, reinterpret_cast<uint2*>((uint32_t*)d_staging)};
+        sort_slice(cfg, cap ? cap : SORT_CAP, d_sc, sb, (uint32_t)gpu.sm_count(), s);
+        uint32_t ctrl[4];
+        s.DtoH(ctrl, d_ctrl, 16);
+        s.DtoH(counts, d_counts, nslots * 4);
+        s.DtoH(offsets, d_offsets, nslots * 4);
+        s.DtoH(sorted, d_sorted, entries * 4);
+        s.sync();
+        std::vector<uint32_t> hl(3 * (size_t)ctrl[1] + 1);
+        if (ctrl[1]) s.DtoH(hl.data(), d_heavy, 12 * (size_t)ctrl[1]);
+        s.sync();
+        for (uint32_t h = 0; h < ctrl[1]; h++) static_cast<uint32_t*>(heavy_slots)[h] = hl[3 * h];
+        info[0] = cfg.nwins; info[1] = cfg.heavy; info[2] = ctrl[1]; info[3] = sort_lg_bins(cfg, n); info[4] = ctrl[3];
+    } catch (const cuda_error& e) {
+        return rust_err(e.code(), e.what());
+    }
+    return rust_ok();
+}

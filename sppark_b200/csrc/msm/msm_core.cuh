@@ -1,10 +1,11 @@
 // Pippenger bucket MSM: per-thread bodies of every kernel on the path, written HD so that
-// tests/emu/msm_emu.cpp can single-step the same logic on the CPU.
+// tests/emu/msm_emu.cpp (the pipeline) and tests/emu/msm_sort_emu.cpp (the bin sort) can
+// single-step the same logic on the CPU.
 //
 // Pipeline (one slice of points, all device-resident):
-//   count      scalars -> signed c-bit digits, histogram per (window, bucket)   [L2 atomics]
-//   scan       per-window exclusive prefix -> bucket offsets, list of heavy buckets
-//   scatter    scalars -> digits again, point index (+sign) into its bucket's slot
+//   sort       scalars -> signed c-bit digits -> (window, bucket) lists of point index (+sign),
+//              bucket counts and offsets, list of heavy buckets; two passes over coarse bins
+//              (bin histogram + partition, then one CTA per bin), see "sort" below
 //   accumulate every lane owns one bucket at a time and streams its points through an XYZZ
 //              mixed add; lanes fetch the next bucket from a global counter the moment they
 //              finish, so a warp never waits for its longest bucket
@@ -85,7 +86,12 @@ struct Digits {
     }
 };
 
-// ---- count / scatter -----------------------------------------------------------------
+// ---- direct sort: one counter and one cursor per (window, bucket) ----------------------------
+// The plain form of the sort below: count every entry into its bucket, exclusive prefix per window,
+// place every entry at its bucket's cursor.  It produces the same counts, offsets and bucket lists
+// (up to the order inside a bucket), and the CPU single-stepper of the whole pipeline
+// (tests/emu/msm_emu.cpp) runs it.  The device does not: with 2^(c-1) buckets per window its
+// random 4-byte stores keep more partly written lines open than L2 holds.
 HD void count_body(const Config& cfg, const uint32_t* scalars, uint32_t* counts, uint32_t i)
 {
     Digits d(scalars + 8 * (size_t)i);
@@ -108,6 +114,88 @@ HD void scatter_body(const Config& cfg, const uint32_t* scalars, uint32_t* curso
             sorted[(size_t)w * cfg.npoints + pos] = i | (neg << 31);
         }
     }
+}
+
+// ---- sort: (window, bucket) lists of point indices -----------------------------------------
+// Two passes over coarse bins, so that no phase writes to more places at once than L2 holds:
+//   bin histogram  bin = (w << lg_bins) + (bucket >> s_w): 2^lg_bins bins per window
+//   partition      every (point, window) entry appended at its bin's cursor in `staging`
+//                  (index | sign << 31, bucket): the open write frontier is one line per bin
+//   bin sort       one CTA per bin: histogram of its 2^s_w buckets in shared memory, counts /
+//                  offsets / heavy buckets, entries placed through shared memory, written out whole
+//   overflow       bins over the CTA's capacity: the same three steps with global atomics
+// Bin b of window w occupies the same range [w*n + bin_base, + bin_count) in `staging` and in
+// `sorted`, since its buckets are consecutive.
+constexpr uint32_t SORT_SMAX = 12;      // a bin spans at most 2^12 buckets (its shared histogram)
+constexpr uint32_t SORT_LG_FILL = 13;   // bins hold about 2^13 entries of a uniform window
+
+// bits of the top window's digit magnitude: bit 255 is ignored, so the window holds bits
+// (W-1)c..254 plus the carry and its buckets are < 2^(255 - (W-1)c) (at most 2^(c-1))
+HD uint32_t top_window_bits(const Config& cfg)
+{
+    const uint32_t e = 255 - (cfg.nwins - 1) * cfg.wbits;
+    return e < cfg.lg_nb ? e : cfg.lg_nb;
+}
+HD uint32_t window_bits(const Config& cfg, uint32_t w) { return w + 1 < cfg.nwins ? cfg.lg_nb : top_window_bits(cfg); }
+// buckets per bin of window w: 2^s_w, so the window's used buckets [0, 2^ub) make <= 2^lg_bins bins
+HD uint32_t bin_shift(const Config& cfg, uint32_t lg_bins, uint32_t w)
+{
+    const uint32_t ub = window_bits(cfg, w);
+    return ub > lg_bins ? ub - lg_bins : 0;
+}
+
+// bins per window for a slice of n points: about 2^SORT_LG_FILL entries per bin, at most 2^SORT_SMAX
+// buckets per bin, at least 4 bins (the bin scan reads them four at a time), at most 2^15 (the bin
+// histogram keeps one window's counters in shared memory); past 2^28 points bins grow instead
+inline uint32_t sort_lg_bins(const Config& cfg, size_t n)
+{
+    int lg_n = 0;
+    while (((size_t)1 << lg_n) < n) lg_n++;
+    int lb = std::max(std::min(lg_n - (int)SORT_LG_FILL, 15), (int)cfg.lg_nb - (int)SORT_SMAX);
+    lb = std::min(lb, (int)cfg.lg_nb);
+    return (uint32_t)std::max(lb, 2);
+}
+
+// bucket range [b0, b0 + nbk) of bin `bin` (window-local) of window w; false for a bin past the
+// window's used buckets (always empty)
+HD bool bin_buckets(const Config& cfg, uint32_t lg_bins, uint32_t w, uint32_t bin, uint32_t& b0, uint32_t& nbk)
+{
+    const uint32_t s = bin_shift(cfg, lg_bins, w), ub = window_bits(cfg, w);
+    b0 = bin << s;
+    nbk = 1u << s;
+    return b0 < (1u << ub);
+}
+
+// the last used bin of a window also owns the offsets of the never-used buckets above it
+HD bool last_bin(const Config& cfg, uint32_t lg_bins, uint32_t w, uint32_t bin)
+{   return ((bin + 1) << bin_shift(cfg, lg_bins, w)) == (1u << window_bits(cfg, w));   }
+
+// every window of point i in order: fn(w, nonzero, bin (global), bucket, entry = i | sign << 31).
+// Windows >= w_end are not visited.  `valid` false: fn sees only zero digits (the tail lanes of a
+// warp that must still take part in its collective operations).
+template<class Fn>
+HD void for_each_digit(const Config& cfg, uint32_t lg_bins, const uint32_t* scalars, uint32_t i, bool valid,
+                       uint32_t w_end, Fn fn)
+{
+    Digits d(scalars + 8 * (size_t)(valid ? i : 0));
+    for (uint32_t w = 0; w < w_end; w++) {
+        uint32_t b, neg;
+        const bool nz = d.next(w, cfg.wbits, b, neg) && valid;
+        fn(w, nz, (w << lg_bins) + (nz ? b >> bin_shift(cfg, lg_bins, w) : 0), b, i | (neg << 31));
+    }
+}
+
+// heavy bucket h: heavy_list[3h] = slot, [3h+1] = first chunk, [3h+2] = #chunks; chunk_map[c] = h
+HD void register_heavy(const Config& cfg, uint32_t t, uint32_t cnt, uint32_t* ctrl, uint32_t* heavy_list,
+                       uint32_t* chunk_map)
+{
+    if (cnt <= cfg.heavy) return;
+    const uint32_t h = atomic_inc(&ctrl[1]), nch = (cnt + cfg.heavy_chunk - 1) / cfg.heavy_chunk;
+    const uint32_t first_chunk = atomic_inc(&ctrl[2], nch);
+    heavy_list[3 * h] = t;
+    heavy_list[3 * h + 1] = first_chunk;
+    heavy_list[3 * h + 2] = nch;
+    for (uint32_t q = 0; q < nch; q++) chunk_map[first_chunk + q] = h;
 }
 
 // ---- point gather -----------------------------------------------------------------------
@@ -301,7 +389,7 @@ inline uint32_t choose_wbits(size_t npoints)
     }
     if (const char* env = getenv("SPPARK_B200_MSM_WBITS")) {
         uint32_t c = (uint32_t)atoi(env);
-        if (c >= 3 && c <= 24) best = c;                 // >= 4 buckets per window (scan_kernel loads uint4)
+        if (c >= 3 && c <= 24) best = c;                 // >= 4 buckets per window (pair_scan_kernel loads uint4)
     }
     return best;
 }
