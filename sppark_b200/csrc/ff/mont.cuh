@@ -221,13 +221,17 @@ struct mont_t {
     // itself inlined into the kernel, so the call depth is one.
 #if defined(__CUDA_ARCH__)
     // ---- double-width arithmetic for the hot loop -----------------------------------------
-    // Products are kept unreduced (2N limbs) so that (a) a squaring can skip the mirrored half
-    // of its partial products, (b) a*b - c*d needs ONE Montgomery reduction, (c) the a*b half
-    // can be split Karatsuba-style.  These trade wide multiplies (the IMAD.WIDE pipe is the busy
-    // one in the MSM) for adds; they are compiled out by default (sppark_b200/build.py).
+    // Products are kept unreduced (2N limbs) so that (a) a*b - c*d needs ONE Montgomery reduction,
+    // (b) the a*b half can be split Karatsuba-style.  These trade wide multiplies (the IMAD.WIDE
+    // pipe is the busy one in the MSM) for adds and a separate reduction pass; they are compiled
+    // out by default (sppark_b200/build.py): on H100 each is slower than the fused ladder in the
+    // BLS12-381 G1 hot loop (DESIGN.md section 7.2).  The squaring instead stays in the fused
+    // ladder (sqr_inline).
     struct wide_t { uint32_t l[2 * N]; };
 
-    // acc += x * v[0..W) at limb position I; even j into the file whose pairs sit at parity(I)
+    // acc += x * v[0..W) at limb position I; even j into the file whose pairs sit at parity(I).
+    // The carry out of each file's chain lands one limb above that file's last pair, which
+    // depends on the parity of W.
     template<int I, int W, class V>
     static DEV void row_w(uint32_t* E, uint32_t* O, uint32_t x, const V& v)
     {
@@ -240,7 +244,7 @@ struct mont_t {
             ptx::madc_lo_cc(A1[I + j], x, v[j], A1[I + j]);
             ptx::madc_hi_cc(A1[I + j + 1], x, v[j], A1[I + j + 1]);
         }
-        ptx::addc(A1[I + W], A1[I + W], 0);
+        ptx::addc(A1[I + W + (W & 1)], A1[I + W + (W & 1)], 0);
         ptx::mad_lo_cc(A2[I + 1], x, v[1], A2[I + 1]);
         ptx::madc_hi_cc(A2[I + 2], x, v[1], A2[I + 2]);
 #pragma unroll
@@ -248,7 +252,7 @@ struct mont_t {
             ptx::madc_lo_cc(A2[I + j], x, v[j], A2[I + j]);
             ptx::madc_hi_cc(A2[I + j + 1], x, v[j], A2[I + j + 1]);
         }
-        ptx::addc(A2[I + W + 1], A2[I + W + 1], 0);
+        ptx::addc(A2[I + W + 1 - (W & 1)], A2[I + W + 1 - (W & 1)], 0);
     }
     template<int I, int W>
     static DEV void mul_rows_w(uint32_t* E, uint32_t* O, const uint32_t* a, const uint32_t* b)
@@ -298,38 +302,39 @@ struct mont_t {
 #if defined(SPPARK_B200_KARATSUBA)
         constexpr bool karatsuba = N % 4 == 0 && N >= 8;
 #else
-        constexpr bool karatsuba = false;   // off: the extra live limbs spill (DESIGN.md section 5)
+        constexpr bool karatsuba = false;   // off: slower on H100 on every curve (DESIGN.md section 7.2)
 #endif
         if constexpr (karatsuba) {
+            // Built in place in t: the differences first (a and b die with the two half products),
+            // then z0 | z2 in t, zm, and the middle term added into t as three carry chains whose
+            // carries out of limb 3H collect in one word.  Live at the peak: t, zm and half of z0.
             constexpr int H = N / 2;
-            uint32_t z0[2 * H], z2[2 * H], zm[2 * H], da[H], db[H];
-            mul_wide_w<H>(z0, a.l, b.l);
-            mul_wide_w<H>(z2, a.l + H, b.l + H);
-            uint32_t sa = abs_diff_w<H>(da, a.l, a.l + H);       // a0 - a1
-            uint32_t sb = abs_diff_w<H>(db, b.l + H, b.l);       // b1 - b0
-            mul_wide_w<H>(zm, da, db);
-            // mid = z0 + z2 +- zm   (2H limbs + a small signed carry word)
-            uint32_t mid[2 * H], top, neg = (sa ^ sb) ? 0xffffffffu : 0u;
-            ptx::add_cc(mid[0], z0[0], z2[0]);
+            uint32_t da[H], db[H], zm[2 * H], z0h[H], top, cf;
+            const uint32_t neg = 0u - (abs_diff_w<H>(da, a.l, a.l + H) ^ abs_diff_w<H>(db, b.l + H, b.l));
+            mul_wide_w<H>(t.l, a.l, b.l);                         // z0 = a0*b0
+            mul_wide_w<H>(t.l + 2 * H, a.l + H, b.l + H);         // z2 = a1*b1
+            mul_wide_w<H>(zm, da, db);                            // |a0 - a1| * |b1 - b0|
 #pragma unroll
-            for (int i = 1; i < 2 * H; i++) ptx::addc_cc(mid[i], z0[i], z2[i]);
+            for (int i = 0; i < H; i++) z0h[i] = t.l[H + i];
+            // += z2 << 32H: limb 2H + i is read before this chain overwrites it
+            ptx::add_cc(t.l[H], t.l[H], t.l[2 * H]);
+#pragma unroll
+            for (int i = 1; i < 2 * H; i++) ptx::addc_cc(t.l[H + i], t.l[H + i], t.l[2 * H + i]);
             ptx::addc(top, 0, 0);
-            // +-zm as (zm ^ neg) + (neg & 1), with the sign extension -neg in the carry word
-            ptx::add_cc(mid[0], mid[0], neg & 1);
+            // += z0 << 32H
+            ptx::add_cc(t.l[H], t.l[H], t.l[0]);
 #pragma unroll
-            for (int i = 1; i < 2 * H; i++) ptx::addc_cc(mid[i], mid[i], 0);
+            for (int i = 1; i < H; i++) ptx::addc_cc(t.l[H + i], t.l[H + i], t.l[i]);
+#pragma unroll
+            for (int i = 0; i < H; i++) ptx::addc_cc(t.l[2 * H + i], t.l[2 * H + i], z0h[i]);
             ptx::addc(top, top, 0);
-            ptx::add_cc(mid[0], mid[0], zm[0] ^ neg);
+            // +-zm << 32H as (zm ^ neg) + (neg & 1), the sign extension neg going into top;
+            // the carry-in comes from neg + neg, which carries exactly when neg is all ones
+            ptx::add_cc(cf, neg, neg);
 #pragma unroll
-            for (int i = 1; i < 2 * H; i++) ptx::addc_cc(mid[i], mid[i], zm[i] ^ neg);
-            ptx::addc(top, top, neg);                 // top in {0,1,2} after the wrap
-            // assemble: t = z0 | z2, then += mid << (32H)
-#pragma unroll
-            for (int i = 0; i < 2 * H; i++) { t.l[i] = z0[i]; t.l[2 * H + i] = z2[i]; }
-            ptx::add_cc(t.l[H], t.l[H], mid[0]);
-#pragma unroll
-            for (int i = 1; i < 2 * H; i++) ptx::addc_cc(t.l[H + i], t.l[H + i], mid[i]);
-            ptx::addc_cc(t.l[3 * H], t.l[3 * H], top);
+            for (int i = 0; i < 2 * H; i++) ptx::addc_cc(t.l[H + i], t.l[H + i], zm[i] ^ neg);
+            ptx::addc(top, top, neg);                 // in {0, 1, 2}: the middle term is a0*b1 + a1*b0 >= 0
+            ptx::add_cc(t.l[3 * H], t.l[3 * H], top);
 #pragma unroll
             for (int i = 3 * H + 1; i < 2 * N - 1; i++) ptx::addc_cc(t.l[i], t.l[i], 0);
             ptx::addc(t.l[2 * N - 1], t.l[2 * N - 1], 0);
@@ -339,64 +344,59 @@ struct mont_t {
         return t;
     }
 
-    // a^2: off-diagonal products once, doubled, plus the diagonal: N(N+1)/2 wide multiplies
+    // a^2 in the fused ladder: step I adds row I of the square, a_I * (a_I, 2a_{I+1}, ..., 2a_{N-1})
+    // at limb 2I, then reduces limb I exactly as rows<> does.  The square terms of limb I all come
+    // from rows k <= I/2, so they are in place when m_I is formed.  N(N+1)/2 wide multiplies for
+    // the square instead of N^2, with the reduction interleaved as in the product.
+    // d[j] = limb j of 2a (2a < 2^(32N) because p < 2^(32N)/3, see sqr_inline)
     template<int I>
-    static DEV void sqr_rows(uint32_t* E, uint32_t* O, const uint32_t* a)
+    static DEV void sqr_rows(uint32_t* E, uint32_t* O, uint32_t& c, const uint32_t* a, const uint32_t* d)
     {
-        if constexpr (I < N - 1) {
-            // products a_I * a_j, j > I, at limb I + j: j - I odd -> odd position -> file O ...
-            constexpr int n_odd = (N - I) / 2;            // j = I+1, I+3, ...
-            constexpr int n_even = (N - I - 1) / 2;       // j = I+2, I+4, ...
-            {
-                uint32_t* A = ((2 * I + 1) & 1) ? O : E;
-                ptx::mad_lo_cc(A[2 * I + 1], a[I], a[I + 1], A[2 * I + 1]);
-                ptx::madc_hi_cc(A[2 * I + 2], a[I], a[I + 1], A[2 * I + 2]);
+        if constexpr (I < N) {
+            if constexpr (I < N - 1) {
+                uint32_t v[N - I];                    // a_I, then 2a with limbs 0..I cleared
+                v[0] = a[I];
+                v[1] = a[I + 1] << 1;
 #pragma unroll
-                for (int k = 1; k < n_odd; k++) {
-                    ptx::madc_lo_cc(A[2 * I + 1 + 2 * k], a[I], a[I + 1 + 2 * k], A[2 * I + 1 + 2 * k]);
-                    ptx::madc_hi_cc(A[2 * I + 2 + 2 * k], a[I], a[I + 1 + 2 * k], A[2 * I + 2 + 2 * k]);
-                }
-                ptx::addc(A[2 * I + 1 + 2 * n_odd], A[2 * I + 1 + 2 * n_odd], 0);
+                for (int k = 2; k < N - I; k++) v[k] = d[I + k];
+                row_w<2 * I, N - I>(E, O, a[I], v);
+            } else {                                  // a_{N-1}^2 alone, at an even limb: file E
+                ptx::mad_lo_cc(E[2 * I], a[I], a[I], E[2 * I]);
+                ptx::madc_hi_cc(E[2 * I + 1], a[I], a[I], E[2 * I + 1]);
+                ptx::addc(E[2 * I + 2], E[2 * I + 2], 0);
             }
-            if constexpr (n_even > 0) {
-                uint32_t* A = E;                          // even positions 2I+2, 2I+4, ...
-                ptx::mad_lo_cc(A[2 * I + 2], a[I], a[I + 2], A[2 * I + 2]);
-                ptx::madc_hi_cc(A[2 * I + 3], a[I], a[I + 2], A[2 * I + 3]);
-#pragma unroll
-                for (int k = 1; k < n_even; k++) {
-                    ptx::madc_lo_cc(A[2 * I + 2 + 2 * k], a[I], a[I + 2 + 2 * k], A[2 * I + 2 + 2 * k]);
-                    ptx::madc_hi_cc(A[2 * I + 3 + 2 * k], a[I], a[I + 2 + 2 * k], A[2 * I + 3 + 2 * k]);
-                }
-                ptx::addc(A[2 * I + 2 + 2 * n_even], A[2 * I + 2 + 2 * n_even], 0);
-            }
-            sqr_rows<I + 1>(E, O, a);
+            uint32_t m = (E[I] + O[I] + c) * C::M0;
+            row_w<I, N>(E, O, m, modulus_view());
+            uint64_t s = (uint64_t)E[I] + O[I] + c;
+            c = (uint32_t)(s >> 32);
+            sqr_rows<I + 1>(E, O, c, a, d);
         }
     }
-    static DEV wide_t sqr_wide(const mont_t& a)
+    static DEV mont_t sqr_inline(const mont_t& a)
     {
-        wide_t t;
-        uint32_t E[2 * N + 2], O[2 * N + 2];
+        // After step I the two files hold less than sum_{k<=I} a_k 2^(32k) * 2a + p 2^(32(I+1)) <
+        // 3p 2^(32(I+1)); p < 2^(32N)/3 keeps that below 2^(32(I+N+1)), so no row chain carries
+        // out of its last limb (the product ladder needs only p < 2^(32N)/2).  Larger moduli (some
+        // scalar fields) square through the product ladder.
+        if constexpr (C::P(N - 1) >= 0x55555555u) {
+            return mul_inline(a, a);
+        } else {
+            uint32_t E[2 * N + 2], O[2 * N + 2], d[N], c = 0;
 #pragma unroll
-        for (int i = 0; i < 2 * N + 2; i++) E[i] = O[i] = 0;
-        sqr_rows<0>(E, O, a.l);
-        // t = 2 * (E + O)
-        ptx::add_cc(t.l[0], E[0], O[0]);
+            for (int i = 0; i < 2 * N + 2; i++) E[i] = O[i] = 0;
 #pragma unroll
-        for (int i = 1; i < 2 * N - 1; i++) ptx::addc_cc(t.l[i], E[i], O[i]);
-        ptx::addc(t.l[2 * N - 1], E[2 * N - 1], O[2 * N - 1]);
-        ptx::add_cc(t.l[0], t.l[0], t.l[0]);
+            for (int j = 1; j < N; j++) d[j] = __funnelshift_l(a.l[j - 1], a.l[j], 1);
+            sqr_rows<0>(E, O, c, a.l, d);
+            mont_t r;
+            ptx::add_cc(r.l[0], E[N], c);
 #pragma unroll
-        for (int i = 1; i < 2 * N - 1; i++) ptx::addc_cc(t.l[i], t.l[i], t.l[i]);
-        ptx::addc(t.l[2 * N - 1], t.l[2 * N - 1], t.l[2 * N - 1]);
-        // + diagonal a_i^2 at limbs (2i, 2i+1): one carry chain over all 2N limbs
-        ptx::mad_lo_cc(t.l[0], a.l[0], a.l[0], t.l[0]);
-        ptx::madc_hi_cc(t.l[1], a.l[0], a.l[0], t.l[1]);
+            for (int i = 1; i < N; i++) ptx::addc_cc(r.l[i], E[N + i], 0);
+            ptx::add_cc(r.l[0], r.l[0], O[N]);
 #pragma unroll
-        for (int i = 1; i < N; i++) {
-            ptx::madc_lo_cc(t.l[2 * i], a.l[i], a.l[i], t.l[2 * i]);
-            ptx::madc_hi_cc(t.l[2 * i + 1], a.l[i], a.l[i], t.l[2 * i + 1]);
+            for (int i = 1; i < N - 1; i++) ptx::addc_cc(r.l[i], r.l[i], O[N + i]);
+            ptx::addc(r.l[N - 1], r.l[N - 1], O[2 * N - 1]);
+            return final_sub(r);
         }
-        return t;
     }
 
     // x - y + p * 2^(32N): stays non-negative for x, y < p^2
@@ -465,14 +465,7 @@ struct mont_t {
         return mul_inline(a, b);                      // the fused ladder: fewest live limbs
 #endif
     }
-    static __device__ __noinline__ mont_t sqr_shared(mont_t a)
-    {
-#if defined(SPPARK_B200_NO_WIDE_SQR)
-        return mul_inline(a, a);
-#else
-        return redc<1>(sqr_wide(a));
-#endif
-    }
+    static __device__ __noinline__ mont_t sqr_shared(mont_t a) { return sqr_inline(a); }
     // a*b - c*d with a single reduction
     static __device__ __noinline__ mont_t msub_shared(mont_t a, mont_t b, mont_t c, mont_t d)
     {

@@ -1,13 +1,16 @@
 // Integer-issue microbenchmark: what bounds the 384-bit Montgomery ladders?
 // Measures warp-instruction throughput of IMAD.WIDE.U32 carry chains (the MSM inner loop),
 // plain IMAD, and IADD3, per SM per clock.   nvcc -arch=sm_90a -O3 imad_bench.cu -o imad_bench
+// Rates are per clock the SMs actually ran at (clock64() over the kernel's event time), since a
+// power-capped card runs below its nominal clock.
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
 
 template<int MODE>
-__global__ void kern(uint32_t* out, uint32_t a, uint32_t b, int iters)
+__global__ void kern(uint32_t* out, long long* cycles, uint32_t a, uint32_t b, int iters)
 {
+    const long long c0 = clock64();
     uint32_t x0 = threadIdx.x, x1 = a, x2 = b, x3 = a ^ b, x4 = 1, x5 = 2, x6 = 3, x7 = 4;
     for (int i = 0; i < iters; i++) {
 #pragma unroll
@@ -43,30 +46,38 @@ __global__ void kern(uint32_t* out, uint32_t a, uint32_t b, int iters)
         }
     }
     out[blockIdx.x * blockDim.x + threadIdx.x] = x0 ^ x1 ^ x2 ^ x3 ^ x4 ^ x5 ^ x6 ^ x7;
+    if (threadIdx.x == 0) cycles[blockIdx.x] = clock64() - c0;
 }
 
-template<int MODE> void run(const char* name, int instr_per_iter, int sms, double mhz)
+template<int MODE> void run(const char* name, int instr_per_iter, int sms, double nominal_mhz)
 {
     uint32_t* out;
+    long long *cycles, h_cycles[1024];
     cudaMalloc(&out, sms * 8 * 1024 * 4);
+    cudaMalloc(&cycles, sms * 8 * sizeof(long long));
     for (int warps = 4; warps <= 32; warps *= 2) {
         int threads = warps * 32 > 1024 ? 1024 : warps * 32;
         int blocks = sms * (warps * 32 / threads);
         cudaEvent_t e0, e1;
         cudaEventCreate(&e0); cudaEventCreate(&e1);
         int iters = 4096;
-        kern<MODE><<<blocks, threads>>>(out, 3, 5, 16);
+        kern<MODE><<<blocks, threads>>>(out, cycles, 3, 5, 16);
         cudaEventRecord(e0);
-        kern<MODE><<<blocks, threads>>>(out, 3, 5, iters);
+        kern<MODE><<<blocks, threads>>>(out, cycles, 3, 5, iters);
         cudaEventRecord(e1);
         cudaEventSynchronize(e1);
         float ms; cudaEventElapsedTime(&ms, e0, e1);
+        cudaMemcpy(h_cycles, cycles, blocks * sizeof(long long), cudaMemcpyDeviceToHost);
+        double cyc = 0;
+        for (int i = 0; i < blocks; i++) cyc += (double)h_cycles[i] / blocks;
+        const double mhz = cyc / (ms * 1e3);                // one wave: every block spans the kernel
         double winstr = (double)blocks * (threads / 32) * iters * 16.0 * instr_per_iter;
         double per_sm_clk = winstr / (ms * 1e-3) / sms / (mhz * 1e6);
-        printf("%-28s warps/SM=%2d  %.3f ms  %.2f warp-instr/clk/SM (at %.0f MHz nominal)  %.1f G thread-instr/s\n",
-               name, warps, ms, per_sm_clk, mhz, winstr * 32 / (ms * 1e-3) / 1e9);
+        printf("%-28s warps/SM=%2d  %.3f ms  %.2f warp-instr/clk/SM (SM clock %.0f MHz, nominal %.0f)  %.1f G thread-instr/s\n",
+               name, warps, ms, per_sm_clk, mhz, nominal_mhz, winstr * 32 / (ms * 1e-3) / 1e9);
     }
     cudaFree(out);
+    cudaFree(cycles);
 }
 
 int main()
