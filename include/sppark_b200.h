@@ -242,6 +242,13 @@ RustError sppark_b200_msm_sharded(int curve, void *out_jacobian, const void *poi
 typedef struct sppark_b200_msm_ctx sppark_b200_msm_ctx;
 RustError sppark_b200_msm_ctx_create(int curve, const void *points_affine, size_t npoints,
                                      size_t ffi_affine_sz, sppark_b200_msm_ctx **out);
+/* Preloaded points as a precomputed fixed-base table: up to `copies` shifted copies 2^(c*V*k) * P_i
+ * are stored, so that an invoke needs V = ceil(D/K) bucket sets instead of D windows (DESIGN.md
+ * section 5a).  copies = 1 is sppark_b200_msm_ctx_create.  Fails for copies = 0 and for
+ * copies * npoints >= 2^31.  _invoke and _free serve both kinds of context. */
+RustError sppark_b200_msm_ctx_create_precomputed(int curve, const void *points_affine, size_t npoints,
+                                                 size_t ffi_affine_sz, uint32_t copies,
+                                                 sppark_b200_msm_ctx **out);
 RustError sppark_b200_msm_ctx_invoke(sppark_b200_msm_ctx *ctx, void *out_jacobian, const void *scalars,
                                      size_t npoints, int scalars_mont);
 void      sppark_b200_msm_ctx_free(sppark_b200_msm_ctx *ctx);

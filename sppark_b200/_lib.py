@@ -44,6 +44,8 @@ _SIGS = {
     "sppark_b200_msm": [C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t],
     "sppark_b200_msm_ex": [C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int],
     "sppark_b200_msm_ctx_create": [C.c_int, C.c_void_p, C.c_size_t, C.c_size_t, C.POINTER(C.c_void_p)],
+    "sppark_b200_msm_ctx_create_precomputed": [C.c_int, C.c_void_p, C.c_size_t, C.c_size_t, C.c_uint32,
+                                               C.POINTER(C.c_void_p)],
     "sppark_b200_msm_ctx_invoke": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int],
     "sppark_b200_msm_dev": [C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p],
     "sppark_b200_generate_points_dev": [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p],

@@ -10,8 +10,8 @@
     RustError msm_dev_##name(void*, const void*, size_t, const void*, void*);                      \
     RustError gen_points_##name(void*, size_t, void*);                                             \
     RustError combine_##name(void*, const void*, size_t);                                          \
-    RustError msm_preload_##name(const void*, size_t, size_t, bool, void**);                       \
-    RustError msm_resident_##name(void*, const void*, size_t, const void*, bool);
+    RustError msm_preload_##name(const void*, size_t, size_t, bool, void**, uint32_t*, uint32_t*); \
+    RustError msm_resident_##name(void*, const void*, size_t, const void*, bool, uint32_t, uint32_t, size_t);
 CURVE_DECLS(bls12_381) CURVE_DECLS(pallas) CURVE_DECLS(vesta) CURVE_DECLS(bls12_381_g2)
 CURVE_DECLS(bn254) CURVE_DECLS(bls12_377) CURVE_DECLS(bn254_g2) CURVE_DECLS(bls12_377_g2)
 
@@ -20,8 +20,8 @@ struct curve_ops {
     RustError (*dev)(void*, const void*, size_t, const void*, void*);
     RustError (*gen)(void*, size_t, void*);
     RustError (*combine)(void*, const void*, size_t);
-    RustError (*preload)(const void*, size_t, size_t, bool, void**);
-    RustError (*resident)(void*, const void*, size_t, const void*, bool);
+    RustError (*preload)(const void*, size_t, size_t, bool, void**, uint32_t*, uint32_t*);
+    RustError (*resident)(void*, const void*, size_t, const void*, bool, uint32_t, uint32_t, size_t);
     size_t affine_bytes, jacobian_bytes;        // packed {X, Y} and {X, Y, Z}
 };
 #define CURVE_ROW(name, affine, jac)                                                               \
@@ -145,27 +145,46 @@ extern "C" RustError sppark_b200_msm_sharded(int curve, void* out, const void* p
 
 // ---- preloaded points (the reference's msm_t{points, npoints} + invoke(out, scalars),
 // msm/pippenger.cuh:377-390,582-601): the SRS stays on the device, only scalars cross PCIe ------
+// copies > 1: d_points holds the precomputed table (csrc/msm/msm_table.cuh) of width wbits, `copies`
+// copies of the npoints rows, copy-major
 struct sppark_b200_msm_ctx {
     int curve, device;
     void* d_points;
     size_t npoints;
+    uint32_t copies, wbits;
 };
 
-extern "C" RustError sppark_b200_msm_ctx_create(int curve, const void* points, size_t npoints,
-                                                size_t ffi_affine_sz, sppark_b200_msm_ctx** out)
+static RustError ctx_create(int curve, const void* points, size_t npoints, size_t ffi_affine_sz, uint32_t copies,
+                            sppark_b200_msm_ctx** out)
 {
     if (out == nullptr) return rust_err(-(int)cudaErrorInvalidValue, "msm_ctx_create: null output");
     *out = nullptr;
     void* d = nullptr;
     const curve_ops* c = curve_of(curve);
     if (c == nullptr) return rust_err(-(int)cudaErrorInvalidValue, "msm_ctx_create: unknown curve");
+    uint32_t wbits = 0;
     RustError e = c->preload(points, npoints, ffi_affine_sz ? ffi_affine_sz : c->affine_bytes,
-                             ffi_affine_sz > c->affine_bytes, &d);
+                             ffi_affine_sz > c->affine_bytes, &d, &copies, &wbits);
     if (e.code != 0) return e;
     int dev = 0;
     (void)cudaGetDevice(&dev);
-    *out = new sppark_b200_msm_ctx{curve, dev, d, npoints};
+    *out = new sppark_b200_msm_ctx{curve, dev, d, npoints, copies, wbits};
     return rust_ok();
+}
+
+extern "C" RustError sppark_b200_msm_ctx_create(int curve, const void* points, size_t npoints,
+                                                size_t ffi_affine_sz, sppark_b200_msm_ctx** out)
+{   return ctx_create(curve, points, npoints, ffi_affine_sz, 1, out);   }
+
+extern "C" RustError sppark_b200_msm_ctx_create_precomputed(int curve, const void* points, size_t npoints,
+                                                            size_t ffi_affine_sz, uint32_t copies,
+                                                            sppark_b200_msm_ctx** out)
+{
+    if (copies == 0) {
+        if (out) *out = nullptr;
+        return rust_err(-(int)cudaErrorInvalidValue, "msm_ctx_create_precomputed: copies must be >= 1");
+    }
+    return ctx_create(curve, points, npoints, ffi_affine_sz, copies, out);
 }
 
 extern "C" RustError sppark_b200_msm_ctx_invoke(sppark_b200_msm_ctx* ctx, void* out, const void* scalars,
@@ -176,7 +195,8 @@ extern "C" RustError sppark_b200_msm_ctx_invoke(sppark_b200_msm_ctx* ctx, void* 
     int cur = 0;
     (void)cudaGetDevice(&cur);
     if (cur != ctx->device) return rust_err(-(int)cudaErrorInvalidDevice, "msm_ctx_invoke: the points live on another device");
-    return curve_of(ctx->curve)->resident(out, ctx->d_points, npoints, scalars, scalars_mont != 0);
+    return curve_of(ctx->curve)->resident(out, ctx->d_points, npoints, scalars, scalars_mont != 0, ctx->wbits,
+                                          ctx->copies, ctx->npoints);
 }
 
 extern "C" void sppark_b200_msm_ctx_free(sppark_b200_msm_ctx* ctx)

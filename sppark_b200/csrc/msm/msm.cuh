@@ -4,6 +4,7 @@
 #include "../util/gpu.cuh"
 #include "msm_core.cuh"
 #include "msm_pair.cuh"
+#include "msm_table.cuh"
 
 namespace msm {
 
@@ -71,20 +72,21 @@ __device__ uint32_t block_exclusive_scan(uint32_t len, Load load, Visit visit)
 
 // pass 1: bin histogram of the windows [w0, w0 + wpg) of group blockIdx.y in shared memory, one
 // global atomic per non-zero counter per CTA; a warp adds equal bins once (all scalars equal:
-// every lane of the warp hits one counter)
+// every lane of the warp hits one counter).  With a table every digit is walked: its set is w mod V.
 static __global__ void __launch_bounds__(HIST_THREADS)
 bin_hist_kernel(const Config cfg, uint32_t lg_bins, const uint32_t* scalars, uint32_t wpg, uint32_t* bin_count)
 {
     extern __shared__ uint32_t hist[];
     const uint32_t w0 = blockIdx.y * wpg, w1 = min(w0 + wpg, cfg.nwins), nctr = (w1 - w0) << lg_bins;
+    const uint32_t d_end = cfg.copies > 1 ? digit_count(cfg) : w1;
     const uint32_t lane = threadIdx.x & 31;
     for (uint32_t k = threadIdx.x; k < nctr; k += blockDim.x) hist[k] = 0;
     __syncthreads();
     for (uint32_t i0 = blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < cfg.npoints; i0 += gridDim.x * blockDim.x) {
         const uint32_t i = i0 + lane;                               // whole warps iterate together
-        for_each_digit(cfg, lg_bins, scalars, i, i < cfg.npoints, w1,
+        for_each_digit(cfg, lg_bins, scalars, i, i < cfg.npoints, d_end,
                        [&](uint32_t w, bool nz, uint32_t bin, uint32_t, uint32_t) {
-            if (w < w0) return;                                     // the same for the whole warp
+            if (w < w0 || w >= w1) return;                          // the same for the whole warp
             const uint32_t key = nz ? bin - (w0 << lg_bins) : ~0u;
             const uint32_t peers = __match_any_sync(0xffffffffu, key);
             if (nz && lane == __ffs(peers) - 1) atomicAdd(&hist[key], __popc(peers));
@@ -113,14 +115,14 @@ partition_kernel(const Config cfg, uint32_t lg_bins, const uint32_t* scalars, ui
     const uint32_t lane = threadIdx.x & 31;
     for (uint32_t i0 = blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < cfg.npoints; i0 += gridDim.x * blockDim.x) {
         const uint32_t i = i0 + lane;
-        for_each_digit(cfg, lg_bins, scalars, i, i < cfg.npoints, cfg.nwins,
+        for_each_digit(cfg, lg_bins, scalars, i, i < cfg.npoints, digit_count(cfg),
                        [&](uint32_t w, bool nz, uint32_t bin, uint32_t b, uint32_t entry) {
             const uint32_t peers = __match_any_sync(0xffffffffu, nz ? bin : ~0u);
             const uint32_t leader = __ffs(peers) - 1;
             uint32_t pos = 0;
             if (nz && lane == leader) pos = atomicAdd(&bin_cur[bin], __popc(peers));
             pos = __shfl_sync(0xffffffffu, pos, leader) + __popc(peers & ((1u << lane) - 1));
-            if (nz) staging[(size_t)w * cfg.npoints + pos] = make_uint2(entry, b);
+            if (nz) staging[(size_t)w * row_stride(cfg) + pos] = make_uint2(entry, b);
         });
     }
 }
@@ -150,7 +152,7 @@ bin_sort_kernel(const Config cfg, uint32_t lg_bins, uint32_t cap, const uint2* s
     uint32_t *run = sm, *cur = sm + cap;
     for (uint32_t k = threadIdx.x; k < nbk; k += blockDim.x) cur[k] = 0;
     __syncthreads();
-    const uint2* src = staging + (size_t)w * cfg.npoints + base;
+    const uint2* src = staging + (size_t)w * row_stride(cfg) + base;
     for (uint32_t k = threadIdx.x; k < cnt; k += blockDim.x) atomicAdd(&cur[src[k].y - b0], 1);
     __syncthreads();
     block_exclusive_scan(nbk, [&](uint32_t j) { return cur[j]; }, [&](uint32_t j, uint32_t c, uint32_t off) {
@@ -164,7 +166,7 @@ bin_sort_kernel(const Config cfg, uint32_t lg_bins, uint32_t cap, const uint2* s
         run[atomicAdd(&cur[e.y - b0], 1)] = e.x;
     }
     __syncthreads();
-    uint32_t* dst = sorted + (size_t)w * cfg.npoints + base;
+    uint32_t* dst = sorted + (size_t)w * row_stride(cfg) + base;
     for (uint32_t k = threadIdx.x; k < cnt; k += blockDim.x) dst[k] = run[k];
 }
 
@@ -180,7 +182,7 @@ overflow_kernel(const Config cfg, uint32_t lg_bins, const uint2* staging, const 
     const uint32_t lane = threadIdx.x & 31, nov = ctrl[3];
     for (uint32_t o = 0; o < nov; o++) {
         const uint32_t g = overflow[o], w = g >> lg_bins, cnt = bin_count[g];
-        const uint2* src = staging + (size_t)w * cfg.npoints + bin_base[g];
+        const uint2* src = staging + (size_t)w * row_stride(cfg) + bin_base[g];
         uint32_t* row = slots + ((size_t)w << cfg.lg_nb);
         for (uint32_t k0 = blockIdx.x * blockDim.x + (threadIdx.x & ~31u); k0 < cnt; k0 += gridDim.x * blockDim.x) {
             const uint32_t k = k0 + lane;
@@ -191,7 +193,7 @@ overflow_kernel(const Config cfg, uint32_t lg_bins, const uint2* staging, const 
             if (k < cnt && lane == leader) pos = atomicAdd(&row[e.y], __popc(peers));
             if (PLACE) {
                 pos = __shfl_sync(0xffffffffu, pos, leader) + __popc(peers & ((1u << lane) - 1));
-                if (k < cnt) sorted[(size_t)w * cfg.npoints + pos] = e.x;
+                if (k < cnt) sorted[(size_t)w * row_stride(cfg) + pos] = e.x;
             }
         }
     }
@@ -235,7 +237,7 @@ inline bool sort_profile() { const char* e = getenv("SPPARK_B200_MSM_SORT_PROFIL
 inline void sort_slice(const Config& cfg, uint32_t cap, const uint32_t* d_scalars, const SortBufs& s, uint32_t sms,
                        cudaStream_t stream)
 {
-    const uint32_t lg_bins = sort_lg_bins(cfg, cfg.npoints);
+    const uint32_t lg_bins = sort_lg_bins(cfg, row_stride(cfg));
     const size_t nbins = (size_t)cfg.nwins << lg_bins, nslots = (size_t)cfg.nwins << cfg.lg_nb;
     const bool marks = sort_profile();
     CUDA_OK(cudaFuncSetAttribute(bin_hist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, HIST_SMEM_WORDS * 4));
@@ -406,7 +408,7 @@ heavy_chunks_kernel(const Config cfg, const uint32_t* points, const uint32_t* so
     for (uint32_t ch = blockIdx.x; ch < nchunks; ch += gridDim.x) {
         const uint32_t h = chunk_map[ch], t = heavy_list[3 * h], k0 = (ch - heavy_list[3 * h + 1]) * cfg.heavy_chunk;
         const uint32_t cnt = counts[t], k1 = min(k0 + cfg.heavy_chunk, cnt);
-        const uint32_t* run = sorted + (size_t)(t >> cfg.lg_nb) * cfg.npoints + offsets[t];
+        const uint32_t* run = sorted + (size_t)(t >> cfg.lg_nb) * row_stride(cfg) + offsets[t];
         ec::xyzz_t<F> acc;
         acc.set_inf();
         for (uint32_t k = k0 + threadIdx.x; k < k1; k += blockDim.x)
@@ -651,6 +653,44 @@ static __global__ void pack_points_kernel(const uint8_t* in, size_t stride, uint
     }
 }
 
+// ---- precomputed tables (msm_table.cuh) --------------------------------------------------------
+template<class F>
+__global__ void __launch_bounds__(128)
+table_double_kernel(const uint32_t* packed, size_t first, uint32_t n, uint32_t steps, uint32_t copies,
+                    uint32_t* xyzz, uint32_t* zzz)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) table_double_body<F>(packed, first, n, steps, copies, xyzz, zzz, i);
+}
+
+template<class F>
+__global__ void __launch_bounds__(128)
+table_normalize_kernel(const uint32_t* xyzz, const uint32_t* zzz_inv, size_t npoints, size_t first, uint32_t n,
+                       uint32_t nslots, uint32_t* table)
+{
+    const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s < nslots) table_normalize_body<F>(xyzz, zzz_inv, npoints, first, n, table, s);
+}
+
+// copies 1 .. cfg.copies - 1 of the npoints packed rows at d_table (copy 0) into the rows after them.
+// Chunks of at most 2^21 (point, copy) pairs bound the XYZZ scratch (480 MB for 48-byte coordinates).
+template<class F>
+void build_table(uint32_t* d_table, size_t npoints, const Config& cfg, const stream_t& stream)
+{
+    const uint32_t K1 = cfg.copies - 1, steps = cfg.wbits * cfg.nwins;
+    if (K1 == 0 || npoints == 0) return;
+    const size_t chunk = std::min<size_t>(npoints, ((size_t)1 << 21) / K1);
+    dev_ptr_t<uint32_t> xyzz(chunk * K1 * 4 * F::N, stream), zzz(chunk * K1 * F::N, stream);
+    for (size_t first = 0; first < npoints; first += chunk) {
+        const uint32_t n = (uint32_t)std::min(chunk, npoints - first), ns = n * K1;
+        table_double_kernel<F><<<(n + 127) / 128, 128, 0, stream>>>(d_table, first, n, steps, cfg.copies, xyzz, zzz);
+        pair_invert_kernel<F><<<((ns + PAIR_M - 1) / PAIR_M + 127) / 128, 128, 0, stream>>>(zzz, ns);
+        table_normalize_kernel<F><<<(ns + 127) / 128, 128, 0, stream>>>(xyzz, zzz, npoints, first, n, ns, d_table);
+        COUNT_LAUNCH(); COUNT_LAUNCH(); COUNT_LAUNCH();
+        CUDA_OK(cudaGetLastError());
+    }
+}
+
 template<class F>
 class msm_t {
     const gpu_t& gpu;
@@ -690,21 +730,27 @@ public:
     {
         if (total_points >= (1ull << 31))
             throw cuda_error(-(int)cudaErrorInvalidValue, "msm: npoints must be < 2^31");
+        return begin(make_config(total_points), slice_cap, stream);
+    }
+
+    // a given geometry (make_config, or config_for_table for the rows of a precomputed table)
+    Job begin(const Config& cfg, size_t slice_cap, cudaStream_t stream)
+    {
         Job j;
-        j.cfg = make_config(total_points);
+        j.cfg = cfg;
         j.cfg.npoints = (uint32_t)slice_cap;
         j.slice_cap = slice_cap;
         j.nslots = (size_t)j.cfg.nwins << j.cfg.lg_nb;
         j.lg_l = j.cfg.lg_nb > 12 ? j.cfg.lg_nb - 12 : 0;          // <= 4096 running-sum items per window
         j.items1 = j.cfg.nwins << (j.cfg.lg_nb - j.lg_l);
         j.slices_done = 0;
-        const size_t entries = (size_t)j.cfg.nwins * slice_cap;
+        const size_t entries = (size_t)j.cfg.nwins * row_stride(j.cfg);
         const size_t heavy_cap = entries / (j.cfg.heavy + 1) + 1;   // most heavy buckets possible
         const size_t chunk_cap = entries / j.cfg.heavy_chunk + heavy_cap; // most chunks possible
         size_t off = 0;
         auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
         const size_t o_counts = take(j.nslots * 4), o_offsets = take(j.nslots * 4), o_cursor = take(j.nslots * 4);
-        const size_t nbins = (size_t)j.cfg.nwins << sort_lg_bins(j.cfg, slice_cap);
+        const size_t nbins = (size_t)j.cfg.nwins << sort_lg_bins(j.cfg, row_stride(j.cfg));
         const size_t o_bcount = take(nbins * 4), o_bbase = take(nbins * 4), o_bcur = take(nbins * 4), o_over = take(nbins * 4);
         const size_t o_staging = take(entries * 8);
         const size_t o_ctrl = take(16), o_heavy = take(heavy_cap * 12), o_cmap = take(chunk_cap * 4);
@@ -768,7 +814,8 @@ public:
             pair_winbase_kernel<<<1, 32, 0, stream>>>(cfg, j.wintotal, j.winbase);
             // the host does not know how many pair sums this slice has (winbase[nwins], on the
             // device): launches cover the bound, threads past the real total return at once
-            const size_t bound = ((size_t)cfg.nwins * n + std::min<size_t>((size_t)cfg.nwins * n, j.nslots) + 1) / 2;
+            const size_t ent = (size_t)cfg.nwins * row_stride(cfg);
+            const size_t bound = (ent + std::min<size_t>(ent, j.nslots) + 1) / 2;
             const size_t per_launch = (size_t)j.pair_threads * PAIR_K;
             for (size_t o0 = 0; o0 < bound; o0 += per_launch) {
                 const uint32_t nth = (uint32_t)std::min<size_t>(j.pair_threads, (bound - o0 + PAIR_K - 1) / PAIR_K);
@@ -800,8 +847,10 @@ public:
             uint32_t dbg[3];
             CUDA_OK(cudaMemcpyAsync(dbg, j.ctrl, 12, cudaMemcpyDeviceToHost, stream));
             CUDA_OK(cudaStreamSynchronize(stream));
-            fprintf(stderr, "[msm] slice %u n=%u wbits=%u nwins=%u heavy_thr=%u tasks_claimed=%u nheavy=%u nchunks=%u acc_blocks=%u\n",
-                    j.slices_done, cfg.npoints, cfg.wbits, cfg.nwins, cfg.heavy, dbg[0], dbg[1], dbg[2], acc_blocks);
+            fprintf(stderr, "[msm] slice %u n=%u wbits=%u nwins=%u heavy_thr=%u tasks_claimed=%u nheavy=%u nchunks=%u acc_blocks=%u"
+                    " digits=%u sets=%u copies=%u\n",
+                    j.slices_done, cfg.npoints, cfg.wbits, cfg.nwins, cfg.heavy, dbg[0], dbg[1], dbg[2], acc_blocks,
+                    digit_count(cfg), cfg.nwins, cfg.copies);
         }
         j.slices_done++;
     }

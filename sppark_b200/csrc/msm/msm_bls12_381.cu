@@ -79,12 +79,13 @@ extern "C" RustError sppark_b200_selftest_field(int field, int op, size_t n, voi
     }
 }
 
-RustError msm_preload_bls12_381(const void* points, size_t npoints, size_t stride, bool has_flag, void** d_points)
-{   return msm_preload<ff::bls12_381_fp_t>(points, npoints, stride, has_flag, d_points);   }
-RustError msm_resident_bls12_381(void* out, const void* d_points, size_t npoints, const void* scalars, bool mont)
+RustError msm_preload_bls12_381(const void* points, size_t npoints, size_t stride, bool has_flag, void** d_points,
+                                uint32_t* copies, uint32_t* wbits)
+{   return msm_preload<ff::bls12_381_fp_t>(points, npoints, stride, has_flag, d_points, copies, wbits);   }
+RustError msm_resident_bls12_381(void* out, const void* d_points, size_t npoints, const void* scalars, bool mont,
+                                 uint32_t wbits, uint32_t copies, size_t stride)
 {
-    return msm_host<ff::bls12_381_fp_t>(out, nullptr, npoints, scalars, 0, false, mont ? scalars_from_mont<ff::bls12_381_fr_t> : nullptr,
-                      (const uint32_t*)d_points);
+    return msm_resident<ff::bls12_381_fp_t, ff::bls12_381_fr_t>(out, d_points, npoints, scalars, mont, wbits, copies, stride);
 }
 
 // ---- device self-test hook: the MSM's bucket sort alone (tests/test_msm_sort.py) -------------------

@@ -26,10 +26,11 @@ extern "C" RustError mult_pippenger_fp2_inf(void* out, const void* points, size_
                                             const void* scalars, size_t ffi_affine_sz)
 {   return msm_host_bls12_381_g2(out, points, npoints, scalars, ffi_affine_sz, true, false);   }
 
-RustError msm_preload_bls12_381_g2(const void* points, size_t npoints, size_t stride, bool has_flag, void** d_points)
-{   return msm_preload<fp2>(points, npoints, stride, has_flag, d_points);   }
-RustError msm_resident_bls12_381_g2(void* out, const void* d_points, size_t npoints, const void* scalars, bool mont)
+RustError msm_preload_bls12_381_g2(const void* points, size_t npoints, size_t stride, bool has_flag, void** d_points,
+                                   uint32_t* copies, uint32_t* wbits)
+{   return msm_preload<fp2>(points, npoints, stride, has_flag, d_points, copies, wbits);   }
+RustError msm_resident_bls12_381_g2(void* out, const void* d_points, size_t npoints, const void* scalars, bool mont,
+                                    uint32_t wbits, uint32_t copies, size_t stride)
 {
-    return msm_host<fp2>(out, nullptr, npoints, scalars, 0, false, mont ? scalars_from_mont<ff::bls12_381_fr_t> : nullptr,
-                      (const uint32_t*)d_points);
+    return msm_resident<fp2, ff::bls12_381_fr_t>(out, d_points, npoints, scalars, mont, wbits, copies, stride);
 }

@@ -23,10 +23,11 @@ RustError gen_points_bn254_g2(void* d_out, size_t n, void* stream)
 {   return gen_points_dev<g2_gen>(d_out, n, stream);   }
 RustError combine_bn254_g2(void* out, const void* partials, size_t count)
 {   return combine_host<fp2>(out, partials, count);   }
-RustError msm_preload_bn254_g2(const void* points, size_t npoints, size_t stride, bool has_flag, void** d_points)
-{   return msm_preload<fp2>(points, npoints, stride, has_flag, d_points);   }
-RustError msm_resident_bn254_g2(void* out, const void* d_points, size_t npoints, const void* scalars, bool mont)
+RustError msm_preload_bn254_g2(const void* points, size_t npoints, size_t stride, bool has_flag, void** d_points,
+                               uint32_t* copies, uint32_t* wbits)
+{   return msm_preload<fp2>(points, npoints, stride, has_flag, d_points, copies, wbits);   }
+RustError msm_resident_bn254_g2(void* out, const void* d_points, size_t npoints, const void* scalars, bool mont,
+                                uint32_t wbits, uint32_t copies, size_t stride)
 {
-    return msm_host<fp2>(out, nullptr, npoints, scalars, 0, false, mont ? scalars_from_mont<ff::bn254_fr_t> : nullptr,
-                         (const uint32_t*)d_points);
+    return msm_resident<fp2, ff::bn254_fr_t>(out, d_points, npoints, scalars, mont, wbits, copies, stride);
 }

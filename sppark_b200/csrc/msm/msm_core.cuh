@@ -24,15 +24,37 @@
 
 namespace msm {
 
+// Precomputed tables (copies > 1): the points are stored K times, copy k holding 2^(c*V*k) * P_i at
+// row i + k * copy_stride.  Digit w = k*V + v of scalar i then goes to bucket set v with the point
+// of copy k, so V = ceil(D / K) bucket sets and V - 1 Horner steps cover all D digits.  With one
+// copy the digit count D and the bucket-set count are both nwins; everything below loops over
+// the bucket sets ("windows") as before.
 struct Config {
     uint32_t wbits;        // c: window width
-    uint32_t nwins;        // ceil(256 / c)
+    uint32_t nwins;        // bucket sets V: ceil(256 / c) without a table, ceil(D / K) with one
     uint32_t lg_nb;        // c - 1: log2(buckets per window)
     uint32_t npoints;
     uint32_t heavy;        // buckets with more entries go to the cooperative kernel
     uint32_t heavy_chunk;  // entries of a heavy bucket folded by one CTA
     uint32_t merge;        // 0: first slice of points (buckets start empty); 1: add into the buckets
+    uint32_t copies;       // K: copies of the points in the table (1: plain points)
+    uint32_t copy_stride;  // points between two copies: the table's point count, not the slice's
 };
+
+// digits per scalar, D = ceil(256 / c) (equal to nwins without a table)
+HD uint32_t digit_count(const Config& cfg) { return (256 + cfg.wbits - 1) / cfg.wbits; }
+// entries per bucket-set row of `staging` / `sorted`: every copy of every point of the slice
+// (a 32-bit product: a table keeps copies * points < 2^31, the bucket entry's index range)
+HD size_t row_stride(const Config& cfg) { return cfg.copies * cfg.npoints; }
+
+// digit w of point i -> bucket set v = w mod V (returned) and entry (i + (w / V) * copy_stride) | sign << 31
+HD uint32_t digit_slot(const Config& cfg, uint32_t w, uint32_t i, uint32_t neg, uint32_t& entry)
+{
+    if (cfg.copies == 1) { entry = i | (neg << 31); return w; }
+    const uint32_t k = w / cfg.nwins;
+    entry = (i + k * cfg.copy_stride) | (neg << 31);
+    return w - k * cfg.nwins;
+}
 
 HD uint32_t atomic_inc(uint32_t* p, uint32_t v = 1)
 {
@@ -95,23 +117,25 @@ struct Digits {
 HD void count_body(const Config& cfg, const uint32_t* scalars, uint32_t* counts, uint32_t i)
 {
     Digits d(scalars + 8 * (size_t)i);
-    for (uint32_t w = 0; w < cfg.nwins; w++) {
-        uint32_t b, neg;
+    const uint32_t nd = digit_count(cfg);
+    for (uint32_t w = 0; w < nd; w++) {
+        uint32_t b, neg, entry;
         if (d.next(w, cfg.wbits, b, neg))
-            atomic_inc(&counts[((size_t)w << cfg.lg_nb) + b]);
+            atomic_inc(&counts[((size_t)digit_slot(cfg, w, i, neg, entry) << cfg.lg_nb) + b]);
     }
 }
 
-// windows [w0, w1) only: digits below w0 are still walked for their carry
+// digits [w0, w1) only: digits below w0 are still walked for their carry
 HD void scatter_body(const Config& cfg, const uint32_t* scalars, uint32_t* cursor,
                      uint32_t* sorted, uint32_t i, uint32_t w0, uint32_t w1)
 {
     Digits d(scalars + 8 * (size_t)i);
     for (uint32_t w = 0; w < w1; w++) {
-        uint32_t b, neg;
+        uint32_t b, neg, entry;
         if (d.next(w, cfg.wbits, b, neg) && w >= w0) {
-            uint32_t pos = atomic_inc(&cursor[((size_t)w << cfg.lg_nb) + b]);
-            sorted[(size_t)w * cfg.npoints + pos] = i | (neg << 31);
+            const uint32_t v = digit_slot(cfg, w, i, neg, entry);
+            uint32_t pos = atomic_inc(&cursor[((size_t)v << cfg.lg_nb) + b]);
+            sorted[(size_t)v * row_stride(cfg) + pos] = entry;
         }
     }
 }
@@ -136,7 +160,9 @@ HD uint32_t top_window_bits(const Config& cfg)
     const uint32_t e = 255 - (cfg.nwins - 1) * cfg.wbits;
     return e < cfg.lg_nb ? e : cfg.lg_nb;
 }
-HD uint32_t window_bits(const Config& cfg, uint32_t w) { return w + 1 < cfg.nwins ? cfg.lg_nb : top_window_bits(cfg); }
+// with a table the thin top digit shares its bucket set with full-width digits: every set is full
+HD uint32_t window_bits(const Config& cfg, uint32_t w)
+{   return w + 1 < cfg.nwins || cfg.copies > 1 ? cfg.lg_nb : top_window_bits(cfg);   }
 // buckets per bin of window w: 2^s_w, so the window's used buckets [0, 2^ub) make <= 2^lg_bins bins
 HD uint32_t bin_shift(const Config& cfg, uint32_t lg_bins, uint32_t w)
 {
@@ -170,18 +196,20 @@ HD bool bin_buckets(const Config& cfg, uint32_t lg_bins, uint32_t w, uint32_t bi
 HD bool last_bin(const Config& cfg, uint32_t lg_bins, uint32_t w, uint32_t bin)
 {   return ((bin + 1) << bin_shift(cfg, lg_bins, w)) == (1u << window_bits(cfg, w));   }
 
-// every window of point i in order: fn(w, nonzero, bin (global), bucket, entry = i | sign << 31).
-// Windows >= w_end are not visited.  `valid` false: fn sees only zero digits (the tail lanes of a
-// warp that must still take part in its collective operations).
+// every digit of point i in order: fn(set, nonzero, bin (global), bucket, entry), with set and entry
+// from digit_slot (without a table: set = digit index, entry = i | sign << 31).  Digits >= w_end are
+// not visited.  `valid` false: fn sees only zero digits (the tail lanes of a warp that must still
+// take part in its collective operations).
 template<class Fn>
 HD void for_each_digit(const Config& cfg, uint32_t lg_bins, const uint32_t* scalars, uint32_t i, bool valid,
                        uint32_t w_end, Fn fn)
 {
     Digits d(scalars + 8 * (size_t)(valid ? i : 0));
     for (uint32_t w = 0; w < w_end; w++) {
-        uint32_t b, neg;
+        uint32_t b, neg, entry;
         const bool nz = d.next(w, cfg.wbits, b, neg) && valid;
-        fn(w, nz, (w << lg_bins) + (nz ? b >> bin_shift(cfg, lg_bins, w) : 0), b, i | (neg << 31));
+        const uint32_t v = digit_slot(cfg, w, i, neg, entry);
+        fn(v, nz, (v << lg_bins) + (nz ? b >> bin_shift(cfg, lg_bins, v) : 0), b, entry);
     }
 }
 
@@ -293,7 +321,7 @@ HD void accumulate_body(const Config& cfg, const uint32_t* points, const uint32_
                 direct_base = winbase[t >> cfg.lg_nb] + off1[t];
             }
             if (live) {
-                if (!DIRECT) run = sorted + (size_t)(t >> cfg.lg_nb) * cfg.npoints + offsets[t];
+                if (!DIRECT) run = sorted + (size_t)(t >> cfg.lg_nb) * row_stride(cfg) + offsets[t];
                 if (cfg.merge) acc = load_bucket<F>(buckets, t);
                 else acc.set_inf();
                 k = 0;
@@ -352,7 +380,8 @@ HD void combine_body(const uint32_t* inR, const uint32_t* inS, uint32_t G, uint3
     store_bucket<F>(outS, item, acc);
 }
 
-// finish: out = sum_w 2^(c*w) * R_w, as a Jacobian point with canonical coordinates
+// finish: out = sum_w 2^(c*w) * R_w over the nwins bucket sets, as a Jacobian point with canonical
+// coordinates (with a table, set v holds every digit v + kV, its factor 2^(cVk) already in the points)
 template<class F>
 HD void finish_body(const Config& cfg, const uint32_t* winR, uint32_t* out_jacobian)
 {
@@ -394,6 +423,21 @@ inline uint32_t choose_wbits(size_t npoints)
     return best;
 }
 
+// a bucket is "heavy" when one lane folding it alone would take longer than that lane's fair
+// share of the whole job (57k lanes: the resident lane count the constant was chosen for; an
+// H100 keeps ~51k resident, close enough for a threshold): such buckets are cut into chunks
+// and spread over CTAs.  At 2^26 points the share is ~15k entries (nothing is heavy for uniform
+// scalars, the long top-window buckets are simply queued first); at 2^16 it is ~25, and the
+// three 16k-entry buckets of the top window must not be left to three single lanes.
+// `entries`: (point, digit) entries of the whole job, D * npoints.
+inline void set_heavy(Config& cfg, uint64_t entries)
+{
+    const uint64_t share = entries / 57000;
+    cfg.heavy = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(share, 256), 16384);
+    cfg.heavy_chunk = std::min<uint32_t>(std::max<uint32_t>(4 * cfg.heavy, 2048), 16384);
+    if (const char* env = getenv("SPPARK_B200_MSM_HEAVY")) cfg.heavy = (uint32_t)atoi(env);
+}
+
 inline Config make_config(size_t npoints)
 {
     Config cfg;
@@ -401,18 +445,50 @@ inline Config make_config(size_t npoints)
     cfg.nwins = (256 + cfg.wbits - 1) / cfg.wbits;
     cfg.lg_nb = cfg.wbits - 1;
     cfg.npoints = (uint32_t)npoints;
-    // a bucket is "heavy" when one lane folding it alone would take longer than that lane's fair
-    // share of the whole job (57k lanes: the resident lane count the constant was chosen for; an
-    // H100 keeps ~51k resident, close enough for a threshold): such buckets are cut into chunks
-    // and spread over CTAs.  At 2^26 points the share is ~15k entries (nothing is heavy for uniform
-    // scalars, the long top-window buckets are simply queued first); at 2^16 it is ~25, and the
-    // three 16k-entry buckets of the top window must not be left to three single lanes.
-    const uint64_t share = (uint64_t)cfg.nwins * npoints / 57000;
-    cfg.heavy = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(share, 256), 16384);
-    cfg.heavy_chunk = std::min<uint32_t>(std::max<uint32_t>(4 * cfg.heavy, 2048), 16384);
     cfg.merge = 0;
-    if (const char* env = getenv("SPPARK_B200_MSM_HEAVY")) cfg.heavy = (uint32_t)atoi(env);
+    cfg.copies = 1;
+    cfg.copy_stride = (uint32_t)npoints;
+    set_heavy(cfg, (uint64_t)cfg.nwins * npoints);
     return cfg;
+}
+
+// ---- precomputed tables ---------------------------------------------------------------------
+// The geometry of a table of width c built for at most `copies` copies: V = ceil(D / K) bucket sets,
+// K_used = ceil(D / V) <= K copies stored (more would add no set), for an MSM over n points of a
+// table whose copies are `stride` points apart.  The heavy threshold follows the D * n entries.
+inline Config config_for_table(size_t n, uint32_t wbits, uint32_t copies, size_t stride)
+{
+    Config cfg;
+    const uint32_t D = (256 + wbits - 1) / wbits, K = std::max(1u, std::min(copies, D));
+    cfg.wbits = wbits;
+    cfg.nwins = (D + K - 1) / K;
+    cfg.lg_nb = wbits - 1;
+    cfg.npoints = (uint32_t)n;
+    cfg.merge = 0;
+    cfg.copies = (D + cfg.nwins - 1) / cfg.nwins;
+    cfg.copy_stride = (uint32_t)stride;
+    set_heavy(cfg, (uint64_t)D * n);
+    return cfg;
+}
+
+// N points, at most K copies: make_config for K = 1; otherwise the width c in [4, 24] minimising the
+// window cost model of choose_wbits re-scored for the table, 1.11 D N + 5.5 V 2^(c-1) (the mixed
+// adds stay D N, the bucket work is paid once per set).  SPPARK_B200_MSM_WBITS overrides c.
+inline Config make_config_precomputed(size_t npoints, uint32_t copies)
+{
+    if (copies <= 1) return make_config(npoints);
+    uint32_t best = 4;
+    double best_cost = 1e300;
+    for (uint32_t c = 4; c <= 24; c++) {
+        const uint32_t D = (256 + c - 1) / c, V = (D + copies - 1) / copies;
+        const double cost = 1.11 * (double)D * (double)npoints + 5.5 * (double)V * (double)(1u << (c - 1));
+        if (cost < best_cost) { best_cost = cost; best = c; }
+    }
+    if (const char* env = getenv("SPPARK_B200_MSM_WBITS")) {
+        uint32_t c = (uint32_t)atoi(env);
+        if (c >= 3 && c <= 24) best = c;
+    }
+    return config_for_table(npoints, best, copies, npoints);
 }
 
 }  // namespace msm

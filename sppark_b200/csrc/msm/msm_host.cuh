@@ -42,10 +42,12 @@ typedef void (*unmont_fn)(uint32_t*, size_t, cudaStream_t);
 // `resident` != nullptr: the points are already on the device as packed affine rows (preloaded by
 // msm_preload below -- the reference's msm_t{points, npoints} constructor + invoke(out, scalars),
 // msm/pippenger.cuh:377-390,582-601): only the scalars cross PCIe, sliced the same way.
+// `table` (with `resident`): the rows are a precomputed table of that width and copy count, whose
+// copies lie table->copy_stride rows apart; slice k's points start at row `first` of every copy.
 template<class F>
 RustError msm_host(void* out, const void* points, size_t npoints, const void* scalars,
                    size_t stride, bool has_flag, unmont_fn unmont = nullptr,
-                   const uint32_t* resident = nullptr)
+                   const uint32_t* resident = nullptr, const msm::Config* table = nullptr)
 {
     constexpr size_t PB = 2 * F::N * 4, JB = 3 * F::N * 4;
     try {
@@ -125,7 +127,9 @@ RustError msm_host(void* out, const void* points, size_t npoints, const void* sc
         } drain{compute, copy};
 
         msm::msm_t<F> m(gpu);
-        auto job = m.begin(npoints, slice_n, compute);
+        auto job = table ? m.begin(msm::config_for_table(npoints, table->wbits, table->copies, table->copy_stride),
+                                   slice_n, compute)
+                         : m.begin(npoints, slice_n, compute);
         size_t first = 0;
         for (size_t k = 0; k < nslices; first += sched[k], k++) {
             const size_t b = k & (nbuf - 1), n = sched[k];
@@ -166,9 +170,13 @@ RustError msm_host(void* out, const void* points, size_t npoints, const void* sc
     return rust_ok();
 }
 
-// host points -> a plain cudaMalloc'ed buffer of packed affine rows that outlives the call
+// host points -> a plain cudaMalloc'ed buffer of packed affine rows that outlives the call.
+// `copies` != nullptr and *copies > 1: the buffer becomes the precomputed table of
+// make_config_precomputed(npoints, *copies) (msm_table.cuh, copy-major rows); *copies and *wbits
+// return the copy count stored and the width the table was built for.
 template<class F>
-RustError msm_preload(const void* points, size_t npoints, size_t stride, bool has_flag, void** d_out)
+RustError msm_preload(const void* points, size_t npoints, size_t stride, bool has_flag, void** d_out,
+                      uint32_t* copies = nullptr, uint32_t* wbits = nullptr)
 {
     constexpr size_t PB = 2 * F::N * 4;
     *d_out = nullptr;
@@ -181,9 +189,15 @@ RustError msm_preload(const void* points, size_t npoints, size_t stride, bool ha
             return rust_err(-(int)cudaErrorInvalidValue, "msm: affine stride must be a multiple of 4 bytes");
         if (npoints >= (1ull << 31))
             return rust_err(-(int)cudaErrorInvalidValue, "msm: npoints must be < 2^31");
+        const uint32_t want = copies ? *copies : 1;
+        if (want == 0)
+            return rust_err(-(int)cudaErrorInvalidValue, "msm: a precomputed table needs at least one copy");
+        if ((uint64_t)want * npoints >= (1ull << 31))      // a bucket entry keeps 31 bits of row index
+            return rust_err(-(int)cudaErrorInvalidValue, "msm: copies * npoints must be < 2^31");
+        const msm::Config tcfg = want > 1 && npoints ? msm::make_config_precomputed(npoints, want) : msm::make_config(npoints);
         const stream_t& copy = gpu[1];
         uint32_t* d_points = nullptr;
-        CUDA_OK(cudaMalloc((void**)&d_points, npoints ? npoints * PB : 1));
+        CUDA_OK(cudaMalloc((void**)&d_points, npoints ? tcfg.copies * npoints * PB : 1));
         struct guard_t { uint32_t* p; ~guard_t() { if (p) (void)cudaFree(p); } } guard{d_points};
         const bool pageable = stager_t::is_pageable(points);
         std::unique_lock<std::mutex> stage_lock(gpu.stage_mtx, std::defer_lock);
@@ -208,15 +222,30 @@ RustError msm_preload(const void* points, size_t npoints, size_t stride, bool ha
             }
             copy.sync();
         }
+        msm::build_table<F>(d_points, npoints, tcfg, copy);
         copy.sync();
         guard.p = nullptr;
         *d_out = d_points;
+        if (copies) { *copies = tcfg.copies; *wbits = tcfg.wbits; }
     } catch (const cuda_error& e) {
         return rust_err(e.code(), e.what());
     } catch (const std::exception& e) {
         return rust_err(-1, e.what());
     }
     return rust_ok();
+}
+
+// MSM of host scalars against the first npoints rows of a msm_preload buffer; wbits / copies /
+// copy_stride: the table it holds (copies = 1: plain rows, the window width follows npoints)
+template<class F, class Fr>
+RustError msm_resident(void* out, const void* d_points, size_t npoints, const void* scalars, bool mont,
+                       uint32_t wbits, uint32_t copies, size_t copy_stride)
+{
+    const unmont_fn unmont = mont ? scalars_from_mont<Fr> : nullptr;
+    if (copies <= 1)
+        return msm_host<F>(out, nullptr, npoints, scalars, 0, false, unmont, (const uint32_t*)d_points);
+    const msm::Config table = msm::config_for_table(copy_stride, wbits, copies, copy_stride);
+    return msm_host<F>(out, nullptr, npoints, scalars, 0, false, unmont, (const uint32_t*)d_points, &table);
 }
 
 template<class F>

@@ -65,7 +65,7 @@ template<class F>
 HD PairTerm<F> pair_term(const Config& cfg, const uint32_t* points, const uint32_t* sorted,
                          const uint32_t* offsets, const uint32_t* counts, PairCursor c)
 {
-    const uint32_t* run = sorted + (size_t)(c.t >> cfg.lg_nb) * cfg.npoints + offsets[c.t];
+    const uint32_t* run = sorted + (size_t)(c.t >> cfg.lg_nb) * row_stride(cfg) + offsets[c.t];
     PairTerm<F> r;
     r.p1 = load_point<F>(points, run[2 * c.i]);
     r.d = F::one();
@@ -110,7 +110,7 @@ template<class F>
 HD F pair_denominator(const Config& cfg, const uint32_t* points, const uint32_t* sorted,
                       const uint32_t* offsets, const uint32_t* counts, PairCursor c)
 {
-    const uint32_t* run = sorted + (size_t)(c.t >> cfg.lg_nb) * cfg.npoints + offsets[c.t];
+    const uint32_t* run = sorted + (size_t)(c.t >> cfg.lg_nb) * row_stride(cfg) + offsets[c.t];
     if (2 * c.i + 1 >= counts[c.t]) return F::one();
     const uint32_t e1 = run[2 * c.i], e2 = run[2 * c.i + 1];
     const F x1 = load_coord<F>(points, e1, 0), x2 = load_coord<F>(points, e2, 0);

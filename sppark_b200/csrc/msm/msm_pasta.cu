@@ -28,18 +28,20 @@ RustError combine_pallas(void* out, const void* partials, size_t count)
 RustError combine_vesta(void* out, const void* partials, size_t count)
 {   return combine_host<ff::vesta_fp_t>(out, partials, count);   }
 
-RustError msm_preload_pallas(const void* points, size_t npoints, size_t stride, bool has_flag, void** d_points)
-{   return msm_preload<ff::pallas_fp_t>(points, npoints, stride, has_flag, d_points);   }
-RustError msm_resident_pallas(void* out, const void* d_points, size_t npoints, const void* scalars, bool mont)
+RustError msm_preload_pallas(const void* points, size_t npoints, size_t stride, bool has_flag, void** d_points,
+                             uint32_t* copies, uint32_t* wbits)
+{   return msm_preload<ff::pallas_fp_t>(points, npoints, stride, has_flag, d_points, copies, wbits);   }
+RustError msm_resident_pallas(void* out, const void* d_points, size_t npoints, const void* scalars, bool mont,
+                              uint32_t wbits, uint32_t copies, size_t stride)
 {
-    return msm_host<ff::pallas_fp_t>(out, nullptr, npoints, scalars, 0, false, mont ? scalars_from_mont<ff::vesta_fp_t> : nullptr,
-                      (const uint32_t*)d_points);
+    return msm_resident<ff::pallas_fp_t, ff::vesta_fp_t>(out, d_points, npoints, scalars, mont, wbits, copies, stride);
 }
 
-RustError msm_preload_vesta(const void* points, size_t npoints, size_t stride, bool has_flag, void** d_points)
-{   return msm_preload<ff::vesta_fp_t>(points, npoints, stride, has_flag, d_points);   }
-RustError msm_resident_vesta(void* out, const void* d_points, size_t npoints, const void* scalars, bool mont)
+RustError msm_preload_vesta(const void* points, size_t npoints, size_t stride, bool has_flag, void** d_points,
+                            uint32_t* copies, uint32_t* wbits)
+{   return msm_preload<ff::vesta_fp_t>(points, npoints, stride, has_flag, d_points, copies, wbits);   }
+RustError msm_resident_vesta(void* out, const void* d_points, size_t npoints, const void* scalars, bool mont,
+                             uint32_t wbits, uint32_t copies, size_t stride)
 {
-    return msm_host<ff::vesta_fp_t>(out, nullptr, npoints, scalars, 0, false, mont ? scalars_from_mont<ff::pallas_fp_t> : nullptr,
-                      (const uint32_t*)d_points);
+    return msm_resident<ff::vesta_fp_t, ff::pallas_fp_t>(out, d_points, npoints, scalars, mont, wbits, copies, stride);
 }

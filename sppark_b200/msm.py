@@ -72,17 +72,27 @@ def msm(curve, points, scalars, mont=False):
 
 class MsmContext:
     """Points preloaded on the current GPU (the reference's msm_t{points, npoints}): every
-    `invoke(scalars)` moves only the scalars.  Host arrays as for msm()."""
+    `invoke(scalars)` moves only the scalars.  Host arrays as for msm().
 
-    def __init__(self, curve, points):
+    precompute=K (an integer >= 1): store up to K shifted copies 2^(c*V*k) * P of the points, a
+    fixed-base table that folds the scalar's D digits into V = ceil(D/K) bucket sets (DESIGN.md
+    section 5a); it takes up to K times the device memory of the points."""
+
+    def __init__(self, curve, points, precompute=None):
         import ctypes as C
         if points.dtype != np.uint64 or not points.flags["C_CONTIGUOUS"]:
             raise TypeError("points must be a C-contiguous uint64 limb array")
         nl = _LIMBS[curve]
         assert points.shape[1] in (2 * nl, 2 * nl + 1)
         self.curve, self.npoints, self._h = curve, points.shape[0], C.c_void_p()
-        _lib.check(_lib.lib().sppark_b200_msm_ctx_create(curve, points.ctypes.data, points.shape[0],
-                                                         points.strides[0], C.byref(self._h)))
+        if precompute is None:
+            err = _lib.lib().sppark_b200_msm_ctx_create(curve, points.ctypes.data, points.shape[0],
+                                                        points.strides[0], C.byref(self._h))
+        else:
+            err = _lib.lib().sppark_b200_msm_ctx_create_precomputed(curve, points.ctypes.data, points.shape[0],
+                                                                    points.strides[0], int(precompute),
+                                                                    C.byref(self._h))
+        _lib.check(err)
 
     def invoke(self, scalars, mont=False):
         if scalars.dtype != np.uint64 or scalars.ndim != 2 or scalars.shape[1] != 4 or not scalars.flags["C_CONTIGUOUS"]:
