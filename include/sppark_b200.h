@@ -267,7 +267,9 @@ RustError sppark_b200_msm_combine(int curve, void *out_jacobian, const void *par
 
 /* device self-test hook for the known-answer tests: r[i] = a[i] (op) b[i] through the PTX field
  * arithmetic; field 0 = BLS12-381 fp (48 B), 1 = BLS12-381 fr, 2 = Pallas fp, 3 = Vesta fp
- * (32 B each); op 0 mul (Montgomery), 1 add, 2 sub, 3 sqr.  Host arrays. */
+ * (32 B each); op 0 mul (Montgomery), 1 add, 2 sub, 3 sqr, 4 mul_shared, 5 sqr_shared,
+ * 6 msub_shared(a, b, b, a^2), 7 msub_shared with four operands: a = (a_i, c_i), b = (b_i, d_i)
+ * interleaved (2n elements each), r[i] = a_i*b_i - c_i*d_i.  Host arrays. */
 RustError sppark_b200_selftest_field(int field, int op, size_t n, void *r, const void *a, const void *b);
 /* same for the single-word NTT fields (SPPARK_FIELD_GL64: 8-byte words, SPPARK_FIELD_BB31: 4-byte
  * Montgomery words): op 0 mul (Goldilocks: b is a canonical constant in Montgomery form, the result

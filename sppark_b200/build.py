@@ -13,10 +13,10 @@ LIB = os.environ.get("SPPARK_B200_LIB") or os.path.join(HERE, "libsppark_b200.so
 
 SOURCES = ["api.cu", "util/gpu.cu", "ntt/ntt.cu", "ntt/ntt_warp.cu", "poly/poly.cu", "msm/msm.cu", "msm/msm_bls12_381.cu", "msm/msm_bls12_381_g2.cu",
            "msm/msm_pasta.cu", "msm/msm_bn254_bls12_377.cu", "msm/msm_bn254_g2.cu", "msm/msm_bls12_377_g2.cu"]
-# the wide-product variants of the hot-loop multiplications (single-reduction a*b - c*d, Karatsuba;
-# ff/mont.cuh) are compiled out: on H100 each made the BLS12-381 G1 accumulate kernel slower than
-# the fused ladder (DESIGN.md section 7.2).  Squaring uses the fused ladder's own squaring form
-NVCC_FLAGS = ["-std=c++17", "-O3", "-DSPPARK_B200_NO_WIDE_MSUB", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
+# the Karatsuba product of the hot loop (ff/mont.cuh, SPPARK_B200_KARATSUBA) stays compiled out: on
+# H100 it made the BLS12-381 G1 accumulate kernel slower than the fused ladder (DESIGN.md section
+# 7.2).  Squaring and a*b - c*d use the fused ladder's own forms
+NVCC_FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "--threads", "4"]
 
 

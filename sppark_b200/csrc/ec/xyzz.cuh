@@ -126,21 +126,21 @@ template<class F> struct xyzz_t {
 
 
     // ---- variants for the bucket-reduction kernels: the same formulae with every product going
-    // through the ONE shared copy of the Montgomery ladder (F::mul_shared) and the point routine
-    // itself inlined, exactly like madd().  The plain add()/dbl() above inline fourteen ladders
-    // (~100 KB of code): fine for cold code, but the running-sum kernels then stall on
-    // instruction fetch (they ran at 40 % of the accumulate kernel's per-product rate).
+    // through the shared copies of the Montgomery ladder (F::mul_shared / sqr_shared / msub_shared)
+    // and the point routine itself inlined, exactly like madd().  The plain add()/dbl() above
+    // inline fourteen ladders (~100 KB of code): fine for cold code, but the running-sum kernels
+    // then stall on instruction fetch (they ran at 40 % of the accumulate kernel's per-product rate).
     HD void dbl_hot()
     {
         if (is_inf()) return;
         F U = Y.dbl();
-        F V = F::mul_shared(U, U);
+        F V = F::sqr_shared(U);
         F W = F::mul_shared(U, V);
         F S = F::mul_shared(X, V);
-        F M = F::mul_shared(X, X);
+        F M = F::sqr_shared(X);
         M = M.dbl() + M;
-        F X3 = F::mul_shared(M, M) - S - S;
-        Y = F::mul_shared(M, S - X3) - F::mul_shared(W, Y);
+        F X3 = F::sqr_shared(M) - S - S;
+        Y = F::msub_shared(M, S - X3, W, Y);
         X = X3;
         ZZ = F::mul_shared(ZZ, V);
         ZZZ = F::mul_shared(ZZZ, W);
@@ -158,11 +158,11 @@ template<class F> struct xyzz_t {
             else set_inf();
             return;
         }
-        F PP = F::mul_shared(P, P);
+        F PP = F::sqr_shared(P);
         F PPP = F::mul_shared(P, PP);
         F Q = F::mul_shared(U1, PP);
-        F X3 = F::mul_shared(R, R) - PPP - Q - Q;
-        Y = F::mul_shared(R, Q - X3) - F::mul_shared(S1, PPP);
+        F X3 = F::sqr_shared(R) - PPP - Q - Q;
+        Y = F::msub_shared(R, Q - X3, S1, PPP);
         X = X3;
         ZZ = F::mul_shared(F::mul_shared(ZZ, p2.ZZ), PP);
         ZZZ = F::mul_shared(F::mul_shared(ZZZ, p2.ZZZ), PPP);

@@ -210,6 +210,24 @@ struct mont_t {
             rows<I + 1>(E, O, c, a, b);
         }
     }
+
+    // a*b - c*d in the same ladder: step I adds the rows a_I * b and c_I * dn, dn = p - d, then
+    // reduces limb I exactly as rows<> does (k is the running carry).  c*dn = -c*d mod p.  a_I and
+    // c_I die with their rows.
+    template<int I>
+    static DEV void msub_rows(uint32_t (&E)[2 * N + 2], uint32_t (&O)[2 * N + 2], uint32_t& k,
+                              const mont_t& a, const mont_t& b, const mont_t& c, const mont_t& dn)
+    {
+        if constexpr (I < N) {
+            row<I>(E, O, a.l[I], b.l);
+            row<I>(E, O, c.l[I], dn.l);
+            uint32_t m = (E[I] + O[I] + k) * C::M0;
+            row<I>(E, O, m, modulus_view());
+            uint64_t s = (uint64_t)E[I] + O[I] + k;
+            k = (uint32_t)(s >> 32);
+            msub_rows<I + 1>(E, O, k, a, b, c, dn);
+        }
+    }
 #endif
 
     friend HD mont_t operator*(const mont_t& a, const mont_t& b) { return mul_inline(a, b); }
@@ -221,12 +239,11 @@ struct mont_t {
     // itself inlined into the kernel, so the call depth is one.
 #if defined(__CUDA_ARCH__)
     // ---- double-width arithmetic for the hot loop -----------------------------------------
-    // Products are kept unreduced (2N limbs) so that (a) a*b - c*d needs ONE Montgomery reduction,
-    // (b) the a*b half can be split Karatsuba-style.  These trade wide multiplies (the IMAD.WIDE
-    // pipe is the busy one in the MSM) for adds and a separate reduction pass; they are compiled
-    // out by default (sppark_b200/build.py): on H100 each is slower than the fused ladder in the
-    // BLS12-381 G1 hot loop (DESIGN.md section 7.2).  The squaring instead stays in the fused
-    // ladder (sqr_inline).
+    // Products kept unreduced (2N limbs), so that a*b can be split Karatsuba-style and reduced in
+    // a separate pass.  That trades wide multiplies (the IMAD.WIDE pipe is the busy one in the
+    // MSM) for adds and the extra pass; it is compiled out by default (SPPARK_B200_KARATSUBA): on
+    // H100 it is slower than the fused ladder in the BLS12-381 G1 hot loop (DESIGN.md section 7.2).
+    // The squaring and a*b - c*d instead stay in the fused ladder (sqr_inline, msub_inline).
     struct wide_t { uint32_t l[2 * N]; };
 
     // acc += x * v[0..W) at limb position I; even j into the file whose pairs sit at parity(I).
@@ -399,22 +416,39 @@ struct mont_t {
         }
     }
 
-    // x - y + p * 2^(32N): stays non-negative for x, y < p^2
-    static DEV wide_t sub_wide(const wide_t& x, const wide_t& y)
+    // a*b - c*d with one reduction, in the fused ladder (msub_rows): 3N^2 wide multiplies instead of
+    // 4N^2.  dn = p - d lies in (0, p] (p when d = 0), so after step I the two files hold less than
+    // (b + dn + p) 2^(32(I+1)) < 3p 2^(32(I+1)), below 2^(32(I+N+1)) when p < 2^(32N)/3 (the
+    // condition of sqr_inline): no row chain carries out of its last limb.  The result is below
+    // (2p^2 + 2^(32N) p) / 2^(32N) < 2p, so one final_sub makes it canonical.  Larger moduli take
+    // two product ladders.
+    static DEV mont_t msub_inline(const mont_t& a, const mont_t& b, const mont_t& c, const mont_t& d)
     {
-        wide_t t;
-        ptx::sub_cc(t.l[0], x.l[0], y.l[0]);
+        if constexpr (C::P(N - 1) >= 0x55555555u) {
+            return mul_inline(a, b) - mul_inline(c, d);
+        } else {
+            mont_t dn;
+            ptx::sub_cc(dn.l[0], C::P(0), d.l[0]);
 #pragma unroll
-        for (int i = 1; i < 2 * N - 1; i++) ptx::subc_cc(t.l[i], x.l[i], y.l[i]);
-        ptx::subc(t.l[2 * N - 1], x.l[2 * N - 1], y.l[2 * N - 1]);
-        ptx::add_cc(t.l[N], t.l[N], C::P(0));
+            for (int i = 1; i < N - 1; i++) ptx::subc_cc(dn.l[i], C::P(i), d.l[i]);
+            ptx::subc(dn.l[N - 1], C::P(N - 1), d.l[N - 1]);
+            uint32_t E[2 * N + 2], O[2 * N + 2], k = 0;
 #pragma unroll
-        for (int i = 1; i < N - 1; i++) ptx::addc_cc(t.l[N + i], t.l[N + i], C::P(i));
-        ptx::addc(t.l[2 * N - 1], t.l[2 * N - 1], C::P(N - 1));
-        return t;
+            for (int i = 0; i < 2 * N + 2; i++) E[i] = O[i] = 0;
+            msub_rows<0>(E, O, k, a, b, c, dn);
+            mont_t r;
+            ptx::add_cc(r.l[0], E[N], k);
+#pragma unroll
+            for (int i = 1; i < N; i++) ptx::addc_cc(r.l[i], E[N + i], 0);
+            ptx::add_cc(r.l[0], r.l[0], O[N]);
+#pragma unroll
+            for (int i = 1; i < N - 1; i++) ptx::addc_cc(r.l[i], r.l[i], O[N + i]);
+            ptx::addc(r.l[N - 1], r.l[N - 1], O[2 * N - 1]);
+            return final_sub(r);
+        }
     }
 
-    // Montgomery reduction of t < K*p*2^(32N) (K = 1 for a product, 2 after sub_wide):
+    // Montgomery reduction of t < K*p*2^(32N) (K = 1 for a product):
     // the multiples m_i*p accumulate in their own even/odd files, limb i of the running total is
     // resolved as an integer carry exactly as in the fused ladder
     template<int I>
@@ -468,13 +502,7 @@ struct mont_t {
     static __device__ __noinline__ mont_t sqr_shared(mont_t a) { return sqr_inline(a); }
     // a*b - c*d with a single reduction
     static __device__ __noinline__ mont_t msub_shared(mont_t a, mont_t b, mont_t c, mont_t d)
-    {
-#if defined(SPPARK_B200_NO_WIDE_MSUB)
-        return mul_inline(a, b) - mul_inline(c, d);
-#else
-        return redc<2>(sub_wide(mul_wide(a, b), mul_wide(c, d)));
-#endif
-    }
+    {   return msub_inline(a, b, c, d);   }
 #else
     static inline mont_t mul_shared(const mont_t& a, const mont_t& b) { return mul_inline(a, b); }
     static inline mont_t sqr_shared(const mont_t& a) { return mul_inline(a, a); }

@@ -23,13 +23,25 @@ extern "C" RustError mult_pippenger_inf(void* out, const void* points, size_t np
 {   return msm_host_bls12_381(out, points, npoints, scalars, ffi_affine_sz, true, false);   }
 
 // ---- device self-test hook: element-wise field ops through the PTX arithmetic -------------
-// op 0 mul, 1 add, 2 sub, 3 sqr, 4 mul_shared, 5 sqr_shared, 6 msub_shared(x,y,y,x^2).  Host arrays of n 48-byte elements.  Used by the GPU KAT tests.
+// op 0 mul, 1 add, 2 sub, 3 sqr, 4 mul_shared, 5 sqr_shared, 6 msub_shared(x,y,y,x^2): host arrays
+// of n elements.  op 7 msub_shared with four independent operands: a = (a_i, c_i) and b = (b_i, d_i)
+// interleaved, 2n elements each, r_i = a_i*b_i - c_i*d_i.  Used by the GPU KAT tests.
 template<class F>
 __global__ void selftest_kernel(int op, size_t n, uint32_t* r, const uint32_t* a, const uint32_t* b)
 {
     size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
     if (i >= n) return;
     F x, y, z;
+    if (op == 7) {
+        F c, d;
+        for (int k = 0; k < F::N; k++) {
+            x.l[k] = a[2 * i * F::N + k]; c.l[k] = a[(2 * i + 1) * F::N + k];
+            y.l[k] = b[2 * i * F::N + k]; d.l[k] = b[(2 * i + 1) * F::N + k];
+        }
+        z = F::msub_shared(x, y, c, d);
+        for (int k = 0; k < F::N; k++) r[i * F::N + k] = z.l[k];
+        return;
+    }
     for (int k = 0; k < F::N; k++) { x.l[k] = a[i * F::N + k]; y.l[k] = b[i * F::N + k]; }
     switch (op) {
     case 0: z = x * y; break;
@@ -49,10 +61,10 @@ static RustError selftest(int op, size_t n, void* r, const void* a, const void* 
     try {
         const gpu_t& gpu = select_gpu(-1);
         const stream_t& s = gpu[0];
-        size_t bytes = n * F::N * 4;
-        dev_ptr_t<uint32_t> da(n * F::N, s), db(n * F::N, s), dr(n * F::N, s);
-        s.HtoD(da, a, bytes);
-        s.HtoD(db, b, bytes);
+        const size_t bytes = n * F::N * 4, in_bytes = op == 7 ? 2 * bytes : bytes;
+        dev_ptr_t<uint32_t> da(in_bytes / 4, s), db(in_bytes / 4, s), dr(n * F::N, s);
+        s.HtoD(da, a, in_bytes);
+        s.HtoD(db, b, in_bytes);
         selftest_kernel<F><<<(unsigned)((n + 127) / 128), 128, 0, s>>>(op, n, dr, da, db);
         COUNT_LAUNCH();
         CUDA_OK(cudaGetLastError());

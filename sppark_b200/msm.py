@@ -152,10 +152,15 @@ def combine(curve, partials):
 
 
 def selftest_field(field, op, a, b):
+    """Element-wise field op on the device, on Montgomery-form rows.  "msub4" takes a = (a_i, c_i)
+    and b = (b_i, d_i) interleaved, 2n rows each, and returns the n rows a_i*b_i - c_i*d_i."""
     a = np.ascontiguousarray(a, dtype=np.uint64)
     b = np.ascontiguousarray(b, dtype=np.uint64)
-    r = np.zeros_like(a)
-    err = _lib.lib().sppark_b200_selftest_field(field, {"mul": 0, "add": 1, "sub": 2, "sqr": 3, "mul_shared": 4, "sqr_shared": 5, "msub_shared": 6}[op],
-                                                a.shape[0], r.ctypes.data, a.ctypes.data, b.ctypes.data)
+    if a.shape != b.shape or (op == "msub4" and a.shape[0] % 2):
+        raise ValueError("selftest_field: operand shapes")
+    n = a.shape[0] // 2 if op == "msub4" else a.shape[0]
+    r = np.zeros((n, a.shape[1]), dtype=np.uint64)
+    ops = {"mul": 0, "add": 1, "sub": 2, "sqr": 3, "mul_shared": 4, "sqr_shared": 5, "msub_shared": 6, "msub4": 7}
+    err = _lib.lib().sppark_b200_selftest_field(field, ops[op], n, r.ctypes.data, a.ctypes.data, b.ctypes.data)
     _lib.check(err)
     return r
