@@ -228,6 +228,14 @@ RustError sppark_b200_msm(int curve, void *out_jacobian, const void *points_affi
 RustError sppark_b200_msm_ex(int curve, void *out_jacobian, const void *points_affine,
                              size_t npoints, const void *scalars, size_t ffi_affine_sz,
                              int scalars_mont);
+/* Same over small scalars: scalar i is the little-endian unsigned integer in bytes
+ * [i * scalar_bytes, (i + 1) * scalar_bytes) (a u32, u64 or u128 array on a little-endian host, or the
+ * 32-byte layout), scalar_bytes = 4, 8, 16 or 32; bits from nbits up are ignored, 1 <= nbits <=
+ * min(255, 8 * scalar_bytes).  Plain integers, no Montgomery flag.  The MSM runs ceil((nbits + 1) / c)
+ * windows instead of ceil(256 / c) and moves scalar_bytes per scalar; nbits = 255 with 32-byte scalars
+ * is sppark_b200_msm_ex(..., 0).  A bad format returns -cudaErrorInvalidValue and infinity. */
+RustError sppark_b200_msm_bits(int curve, void *out_jacobian, const void *points_affine, size_t npoints,
+                               const void *scalars, size_t ffi_affine_sz, uint32_t scalar_bytes, uint32_t nbits);
 /* One MSM sharded by point-chunk over GPUs of this process (SURVEY.md section 8e): chunk i of the points /
  * scalars runs on device_ids[i] through the host-pointer pipeline of that device, the ndev partial
  * results are added on the first device.  ndev = 1..64; ids may repeat (chunks of one device run
@@ -251,12 +259,21 @@ RustError sppark_b200_msm_ctx_create_precomputed(int curve, const void *points_a
                                                  sppark_b200_msm_ctx **out);
 RustError sppark_b200_msm_ctx_invoke(sppark_b200_msm_ctx *ctx, void *out_jacobian, const void *scalars,
                                      size_t npoints, int scalars_mont);
+/* _invoke over small scalars (format as sppark_b200_msm_bits).  A precomputed table keeps its width c
+ * and bucket sets V; only the digits below ceil((nbits + 1) / c), and so only the copies holding them,
+ * are read. */
+RustError sppark_b200_msm_ctx_invoke_bits(sppark_b200_msm_ctx *ctx, void *out_jacobian, const void *scalars,
+                                          size_t npoints, uint32_t scalar_bytes, uint32_t nbits);
 void      sppark_b200_msm_ctx_free(sppark_b200_msm_ctx *ctx);
 /* msm_t::invoke with device-resident points and scalars (msm/pippenger.cuh:582-601):
  * d_points: packed affine {X,Y}; d_scalars: 32-B LE; result written to HOST out_jacobian
  * after synchronising `stream`. */
 RustError sppark_b200_msm_dev(int curve, void *out_jacobian, const void *d_points,
                               size_t npoints, const void *d_scalars, void *stream);
+/* sppark_b200_msm_dev over small scalars (format as sppark_b200_msm_bits); d_scalars must be aligned
+ * to min(scalar_bytes, 16) bytes, each scalar is read with one load of its width. */
+RustError sppark_b200_msm_dev_bits(int curve, void *out_jacobian, const void *d_points, size_t npoints,
+                                   const void *d_scalars, uint32_t scalar_bytes, uint32_t nbits, void *stream);
 
 /* synthetic inputs: d_out[i] = (i+1)*G as packed affine points in DEVICE memory (the role of
  * util::generate_points_scalars, poc/msm-cuda/src/util.rs:11-38); enqueued on `stream`. */

@@ -1,27 +1,31 @@
 // Curve dispatch for the extended MSM entry points (include/sppark_b200.h).
 #include "../util/gpu.cuh"
+#include <cstring>
 #include <thread>
 #include <vector>
 
 // one row per curve id (SPPARK_CURVE_*): the six entry points its translation unit defines
-// (msm_bls12_381.cu, msm_pasta.cu, msm_bn254_bls12_377.cu, msm_*_g2.cu) and its packed layouts
+// (msm_bls12_381.cu, msm_pasta.cu, msm_bn254_bls12_377.cu, msm_*_g2.cu) and its packed layouts.
+// The MSM entries end in the scalar format (scalar_bytes, nbits): 32, 255 for 32-byte scalars.
 #define CURVE_DECLS(name)                                                                          \
-    RustError msm_host_##name(void*, const void*, size_t, const void*, size_t, bool, bool);        \
-    RustError msm_dev_##name(void*, const void*, size_t, const void*, void*);                      \
+    RustError msm_host_##name(void*, const void*, size_t, const void*, size_t, bool, bool,         \
+                              uint32_t, uint32_t);                                                 \
+    RustError msm_dev_##name(void*, const void*, size_t, const void*, void*, uint32_t, uint32_t);  \
     RustError gen_points_##name(void*, size_t, void*);                                             \
     RustError combine_##name(void*, const void*, size_t);                                          \
     RustError msm_preload_##name(const void*, size_t, size_t, bool, void**, uint32_t*, uint32_t*); \
-    RustError msm_resident_##name(void*, const void*, size_t, const void*, bool, uint32_t, uint32_t, size_t);
+    RustError msm_resident_##name(void*, const void*, size_t, const void*, bool, uint32_t, uint32_t, size_t, \
+                                  uint32_t, uint32_t);
 CURVE_DECLS(bls12_381) CURVE_DECLS(pallas) CURVE_DECLS(vesta) CURVE_DECLS(bls12_381_g2)
 CURVE_DECLS(bn254) CURVE_DECLS(bls12_377) CURVE_DECLS(bn254_g2) CURVE_DECLS(bls12_377_g2)
 
 struct curve_ops {
-    RustError (*host)(void*, const void*, size_t, const void*, size_t, bool, bool);
-    RustError (*dev)(void*, const void*, size_t, const void*, void*);
+    RustError (*host)(void*, const void*, size_t, const void*, size_t, bool, bool, uint32_t, uint32_t);
+    RustError (*dev)(void*, const void*, size_t, const void*, void*, uint32_t, uint32_t);
     RustError (*gen)(void*, size_t, void*);
     RustError (*combine)(void*, const void*, size_t);
     RustError (*preload)(const void*, size_t, size_t, bool, void**, uint32_t*, uint32_t*);
-    RustError (*resident)(void*, const void*, size_t, const void*, bool, uint32_t, uint32_t, size_t);
+    RustError (*resident)(void*, const void*, size_t, const void*, bool, uint32_t, uint32_t, size_t, uint32_t, uint32_t);
     size_t affine_bytes, jacobian_bytes;        // packed {X, Y} and {X, Y, Z}
 };
 #define CURVE_ROW(name, affine, jac)                                                               \
@@ -58,12 +62,37 @@ extern "C" RustError sppark_b200_msm_combine(int curve, void* out, const void* p
 
 // ffi_affine_sz: 0 = packed {X, Y}; larger than that = arkworks rows with an infinity flag after Y
 static RustError msm_any(int curve, void* out, const void* points, size_t npoints, const void* scalars,
-                         size_t ffi_affine_sz, bool mont)
+                         size_t ffi_affine_sz, bool mont, uint32_t scalar_bytes = 32, uint32_t nbits = 255)
 {
     const curve_ops* c = curve_of(curve);
     if (c == nullptr) return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_msm: unknown curve");
     return c->host(out, points, npoints, scalars, ffi_affine_sz ? ffi_affine_sz : c->affine_bytes,
-                   ffi_affine_sz > c->affine_bytes, mont);
+                   ffi_affine_sz > c->affine_bytes, mont, scalar_bytes, nbits);
+}
+
+// the scalar format of the _bits entries: 4, 8, 16 or 32 bytes, 1 <= nbits <= min(255, 8 * bytes)
+static bool scalar_format_ok(uint32_t scalar_bytes, uint32_t nbits)
+{
+    const bool width = scalar_bytes == 4 || scalar_bytes == 8 || scalar_bytes == 16 || scalar_bytes == 32;
+    return width && nbits >= 1 && nbits <= 255 && nbits <= 8 * scalar_bytes;
+}
+// a refused call returns infinity, as a failed MSM does
+static RustError refuse(void* out, size_t jacobian_bytes, const char* msg)
+{
+    if (out) memset(out, 0, jacobian_bytes);
+    return rust_err(-(int)cudaErrorInvalidValue, msg);
+}
+
+extern "C" RustError sppark_b200_msm_bits(int curve, void* out, const void* points, size_t npoints,
+                                          const void* scalars, size_t ffi_affine_sz, uint32_t scalar_bytes,
+                                          uint32_t nbits)
+{
+    const curve_ops* c = curve_of(curve);
+    if (c == nullptr) return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_msm_bits: unknown curve");
+    if (!scalar_format_ok(scalar_bytes, nbits))
+        return refuse(out, c->jacobian_bytes, "sppark_b200_msm_bits: scalar_bytes must be 4, 8, 16 or 32 and "
+                                              "1 <= nbits <= min(255, 8 * scalar_bytes)");
+    return msm_any(curve, out, points, npoints, scalars, ffi_affine_sz, false, scalar_bytes, nbits);
 }
 
 extern "C" RustError sppark_b200_msm(int curve, void* out, const void* points, size_t npoints,
@@ -79,7 +108,22 @@ extern "C" RustError sppark_b200_msm_dev(int curve, void* out, const void* d_poi
 {
     const curve_ops* c = curve_of(curve);
     if (c == nullptr) return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_msm_dev: unknown curve");
-    return c->dev(out, d_points, npoints, d_scalars, stream);
+    return c->dev(out, d_points, npoints, d_scalars, stream, 32, 255);
+}
+
+extern "C" RustError sppark_b200_msm_dev_bits(int curve, void* out, const void* d_points, size_t npoints,
+                                              const void* d_scalars, uint32_t scalar_bytes, uint32_t nbits,
+                                              void* stream)
+{
+    const curve_ops* c = curve_of(curve);
+    if (c == nullptr) return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_msm_dev_bits: unknown curve");
+    if (!scalar_format_ok(scalar_bytes, nbits))
+        return refuse(out, c->jacobian_bytes, "sppark_b200_msm_dev_bits: scalar_bytes must be 4, 8, 16 or 32 and "
+                                              "1 <= nbits <= min(255, 8 * scalar_bytes)");
+    if ((uintptr_t)d_scalars % (scalar_bytes < 16 ? scalar_bytes : 16) != 0)   // one aligned load per scalar
+        return refuse(out, c->jacobian_bytes, "sppark_b200_msm_dev_bits: d_scalars must be aligned to "
+                                              "min(scalar_bytes, 16) bytes");
+    return c->dev(out, d_points, npoints, d_scalars, stream, scalar_bytes, nbits);
 }
 
 // ---- one MSM sharded by point-chunk over several GPUs of this process (SURVEY.md section 8e) --------
@@ -196,7 +240,24 @@ extern "C" RustError sppark_b200_msm_ctx_invoke(sppark_b200_msm_ctx* ctx, void* 
     (void)cudaGetDevice(&cur);
     if (cur != ctx->device) return rust_err(-(int)cudaErrorInvalidDevice, "msm_ctx_invoke: the points live on another device");
     return curve_of(ctx->curve)->resident(out, ctx->d_points, npoints, scalars, scalars_mont != 0, ctx->wbits,
-                                          ctx->copies, ctx->npoints);
+                                          ctx->copies, ctx->npoints, 32, 255);
+}
+
+extern "C" RustError sppark_b200_msm_ctx_invoke_bits(sppark_b200_msm_ctx* ctx, void* out, const void* scalars,
+                                                     size_t npoints, uint32_t scalar_bytes, uint32_t nbits)
+{
+    if (ctx == nullptr) return rust_err(-(int)cudaErrorInvalidValue, "msm_ctx_invoke_bits: null context");
+    const curve_ops* c = curve_of(ctx->curve);
+    if (!scalar_format_ok(scalar_bytes, nbits))
+        return refuse(out, c->jacobian_bytes, "msm_ctx_invoke_bits: scalar_bytes must be 4, 8, 16 or 32 and "
+                                              "1 <= nbits <= min(255, 8 * scalar_bytes)");
+    if (npoints > ctx->npoints)
+        return rust_err(-(int)cudaErrorInvalidValue, "msm_ctx_invoke_bits: more scalars than preloaded points");
+    int cur = 0;
+    (void)cudaGetDevice(&cur);
+    if (cur != ctx->device) return rust_err(-(int)cudaErrorInvalidDevice, "msm_ctx_invoke_bits: the points live on another device");
+    return c->resident(out, ctx->d_points, npoints, scalars, false, ctx->wbits, ctx->copies, ctx->npoints,
+                       scalar_bytes, nbits);
 }
 
 extern "C" void sppark_b200_msm_ctx_free(sppark_b200_msm_ctx* ctx)

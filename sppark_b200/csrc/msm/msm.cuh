@@ -73,7 +73,9 @@ __device__ uint32_t block_exclusive_scan(uint32_t len, Load load, Visit visit)
 // pass 1: bin histogram of the windows [w0, w0 + wpg) of group blockIdx.y in shared memory, one
 // global atomic per non-zero counter per CTA; a warp adds equal bins once (all scalars equal:
 // every lane of the warp hits one counter).  With a table every digit is walked: its set is w mod V.
-static __global__ void __launch_bounds__(HIST_THREADS)
+// One instantiation per scalar width SW (cfg.swords words), each scalar read with one load of its width.
+template<uint32_t SW>
+__global__ void __launch_bounds__(HIST_THREADS)
 bin_hist_kernel(const Config cfg, uint32_t lg_bins, const uint32_t* scalars, uint32_t wpg, uint32_t* bin_count)
 {
     extern __shared__ uint32_t hist[];
@@ -84,7 +86,7 @@ bin_hist_kernel(const Config cfg, uint32_t lg_bins, const uint32_t* scalars, uin
     __syncthreads();
     for (uint32_t i0 = blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < cfg.npoints; i0 += gridDim.x * blockDim.x) {
         const uint32_t i = i0 + lane;                               // whole warps iterate together
-        for_each_digit(cfg, lg_bins, scalars, i, i < cfg.npoints, d_end,
+        for_each_digit<SW>(cfg, lg_bins, scalars, i, i < cfg.npoints, d_end,
                        [&](uint32_t w, bool nz, uint32_t bin, uint32_t, uint32_t) {
             if (w < w0 || w >= w1) return;                          // the same for the whole warp
             const uint32_t key = nz ? bin - (w0 << lg_bins) : ~0u;
@@ -109,13 +111,14 @@ bin_scan_kernel(uint32_t lg_bins, const uint32_t* bin_count, uint32_t* bin_base,
 // pass 2: every (point, window) entry appended at its bin's cursor, one reservation per distinct
 // bin per warp.  All windows in one pass: the open frontier is one partly written line per bin
 // (W * 2^lg_bins * 128 B, 13.6 MB at 2^26 points), so lines fill in L2 and leave whole.
-static __global__ void __launch_bounds__(256)
+template<uint32_t SW>
+__global__ void __launch_bounds__(256)
 partition_kernel(const Config cfg, uint32_t lg_bins, const uint32_t* scalars, uint32_t* bin_cur, uint2* staging)
 {
     const uint32_t lane = threadIdx.x & 31;
     for (uint32_t i0 = blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < cfg.npoints; i0 += gridDim.x * blockDim.x) {
         const uint32_t i = i0 + lane;
-        for_each_digit(cfg, lg_bins, scalars, i, i < cfg.npoints, digit_count(cfg),
+        for_each_digit<SW>(cfg, lg_bins, scalars, i, i < cfg.npoints, digit_count(cfg),
                        [&](uint32_t w, bool nz, uint32_t bin, uint32_t b, uint32_t entry) {
             const uint32_t peers = __match_any_sync(0xffffffffu, nz ? bin : ~0u);
             const uint32_t leader = __ffs(peers) - 1;
@@ -233,14 +236,15 @@ inline bool sort_profile() { const char* e = getenv("SPPARK_B200_MSM_SORT_PROFIL
 
 // (window, bucket) lists of cfg.npoints scalars: counts, offsets, sorted, ctrl[1..3], heavy_list,
 // chunk_map.  cap <= SORT_CAP: entries per bin-sort CTA (smaller values send more bins down the
-// overflow path; the self-test uses that).
-inline void sort_slice(const Config& cfg, uint32_t cap, const uint32_t* d_scalars, const SortBufs& s, uint32_t sms,
-                       cudaStream_t stream)
+// overflow path; the self-test uses that).  SW = cfg.swords: the scalar width of d_scalars.
+template<uint32_t SW>
+void sort_slice_sw(const Config& cfg, uint32_t cap, const uint32_t* d_scalars, const SortBufs& s, uint32_t sms,
+                   cudaStream_t stream)
 {
     const uint32_t lg_bins = sort_lg_bins(cfg, row_stride(cfg));
     const size_t nbins = (size_t)cfg.nwins << lg_bins, nslots = (size_t)cfg.nwins << cfg.lg_nb;
     const bool marks = sort_profile();
-    CUDA_OK(cudaFuncSetAttribute(bin_hist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, HIST_SMEM_WORDS * 4));
+    CUDA_OK(cudaFuncSetAttribute(bin_hist_kernel<SW>, cudaFuncAttributeMaxDynamicSharedMemorySize, HIST_SMEM_WORDS * 4));
     CUDA_OK(cudaFuncSetAttribute(bin_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  (SORT_CAP + (1u << SORT_SMAX)) * 4));
     CUDA_OK(cudaMemsetAsync(s.counts, 0, nslots * 4, stream));
@@ -249,14 +253,14 @@ inline void sort_slice(const Config& cfg, uint32_t cap, const uint32_t* d_scalar
     const uint32_t wpg = std::min(cfg.nwins, HIST_SMEM_WORDS >> lg_bins);
     const uint32_t ngroups = (cfg.nwins + wpg - 1) / wpg;
     const uint32_t hist_blk = (uint32_t)std::min<size_t>((cfg.npoints + HIST_THREADS - 1) / HIST_THREADS, sms);
-    bin_hist_kernel<<<dim3(hist_blk, ngroups), HIST_THREADS, ((size_t)wpg << lg_bins) * 4, stream>>>(
+    bin_hist_kernel<SW><<<dim3(hist_blk, ngroups), HIST_THREADS, ((size_t)wpg << lg_bins) * 4, stream>>>(
         cfg, lg_bins, d_scalars, wpg, s.bin_count);
     COUNT_LAUNCH();
     bin_scan_kernel<<<cfg.nwins, 1024, 0, stream>>>(lg_bins, s.bin_count, s.bin_base, s.bin_cur);
     COUNT_LAUNCH();
     if (marks) g_profile.mark("sort_partition", stream);
     const uint32_t part_blk = (uint32_t)std::min<size_t>((cfg.npoints + 255) / 256, (size_t)sms * 8);
-    partition_kernel<<<part_blk, 256, 0, stream>>>(cfg, lg_bins, d_scalars, s.bin_cur, s.staging);
+    partition_kernel<SW><<<part_blk, 256, 0, stream>>>(cfg, lg_bins, d_scalars, s.bin_cur, s.staging);
     COUNT_LAUNCH();
     if (marks) g_profile.mark("sort_bins", stream);
     bin_sort_kernel<<<(uint32_t)nbins, SORT_THREADS, (cap + (1u << SORT_SMAX)) * 4, stream>>>(
@@ -272,6 +276,18 @@ inline void sort_slice(const Config& cfg, uint32_t cap, const uint32_t* d_scalar
                                                        s.overflow, s.cursor, s.sorted);
     COUNT_LAUNCH(); COUNT_LAUNCH(); COUNT_LAUNCH();
     CUDA_OK(cudaGetLastError());
+}
+
+inline void sort_slice(const Config& cfg, uint32_t cap, const uint32_t* d_scalars, const SortBufs& s, uint32_t sms,
+                       cudaStream_t stream)
+{
+    switch (cfg.swords) {
+    case 1: sort_slice_sw<1>(cfg, cap, d_scalars, s, sms, stream); break;
+    case 2: sort_slice_sw<2>(cfg, cap, d_scalars, s, sms, stream); break;
+    case 4: sort_slice_sw<4>(cfg, cap, d_scalars, s, sms, stream); break;
+    case 8: sort_slice_sw<8>(cfg, cap, d_scalars, s, sms, stream); break;
+    default: throw cuda_error(-(int)cudaErrorInvalidValue, "msm: scalars must be 4, 8, 16 or 32 bytes");
+    }
 }
 
 // ---- batched-affine pre-reduction of the bucket lists (msm_pair.cuh) ---------------------------
@@ -725,12 +741,14 @@ public:
         ~Job() { if (blob) (void)cudaFreeAsync(blob, owner); }
     };
 
-    // total_points fixes the window width; slice_cap is the most points one slice() call may carry
-    Job begin(size_t total_points, size_t slice_cap, cudaStream_t stream)
+    // total_points and the scalar format fix the window width (make_config); slice_cap is the most
+    // points one slice() call may carry
+    Job begin(size_t total_points, size_t slice_cap, cudaStream_t stream, uint32_t nbits = 255,
+              uint32_t scalar_bytes = 32)
     {
         if (total_points >= (1ull << 31))
             throw cuda_error(-(int)cudaErrorInvalidValue, "msm: npoints must be < 2^31");
-        return begin(make_config(total_points), slice_cap, stream);
+        return begin(make_config(total_points, nbits, scalar_bytes), slice_cap, stream);
     }
 
     // a given geometry (make_config, or config_for_table for the rows of a precomputed table)
@@ -848,9 +866,9 @@ public:
             CUDA_OK(cudaMemcpyAsync(dbg, j.ctrl, 12, cudaMemcpyDeviceToHost, stream));
             CUDA_OK(cudaStreamSynchronize(stream));
             fprintf(stderr, "[msm] slice %u n=%u wbits=%u nwins=%u heavy_thr=%u tasks_claimed=%u nheavy=%u nchunks=%u acc_blocks=%u"
-                    " digits=%u sets=%u copies=%u\n",
+                    " digits=%u sets=%u copies=%u nbits=%u sbytes=%u\n",
                     j.slices_done, cfg.npoints, cfg.wbits, cfg.nwins, cfg.heavy, dbg[0], dbg[1], dbg[2], acc_blocks,
-                    digit_count(cfg), cfg.nwins, cfg.copies);
+                    digit_count(cfg), cfg.nwins, cfg.copies, (uint32_t)cfg.nbits, 4u * cfg.swords);
         }
         j.slices_done++;
     }
@@ -888,16 +906,16 @@ public:
         j.blob = nullptr;
     }
 
-    // all inputs device-resident: d_points packed affine, d_scalars 8 words each.
-    // d_out: JW words of device memory.  Enqueues on `stream`; no synchronisation.
+    // all inputs device-resident: d_points packed affine, d_scalars scalar_bytes each (bits from nbits
+    // up ignored).  d_out: JW words of device memory.  Enqueues on `stream`; no synchronisation.
     void invoke_dev(uint32_t* d_out, const uint32_t* d_points, size_t npoints,
-                    const uint32_t* d_scalars, cudaStream_t stream)
+                    const uint32_t* d_scalars, cudaStream_t stream, uint32_t nbits = 255, uint32_t scalar_bytes = 32)
     {
         if (npoints == 0) {
             CUDA_OK(cudaMemsetAsync(d_out, 0, JW * 4, stream));
             return;
         }
-        Job j = begin(npoints, npoints, stream);
+        Job j = begin(npoints, npoints, stream, nbits, scalar_bytes);
         slice(j, d_points, d_scalars, npoints, stream);
         finish(j, d_out, stream);
     }

@@ -31,7 +31,7 @@ namespace msm {
 // the bucket sets ("windows") as before.
 struct Config {
     uint32_t wbits;        // c: window width
-    uint32_t nwins;        // bucket sets V: ceil(256 / c) without a table, ceil(D / K) with one
+    uint32_t nwins;        // bucket sets V: D = ceil((nbits + 1) / c) without a table, ceil(D / K) with one
     uint32_t lg_nb;        // c - 1: log2(buckets per window)
     uint32_t npoints;
     uint32_t heavy;        // buckets with more entries go to the cooperative kernel
@@ -39,10 +39,17 @@ struct Config {
     uint32_t merge;        // 0: first slice of points (buckets start empty); 1: add into the buckets
     uint32_t copies;       // K: copies of the points in the table (1: plain points)
     uint32_t copy_stride;  // points between two copies: the table's point count, not the slice's
+    // the scalar format: scalar i is the little-endian integer in words [i * swords, (i + 1) * swords),
+    // bits from nbits up are ignored (255 and 8 words for the 32-byte entries).  Two 16-bit fields fill
+    // the struct's padding, so the kernel parameters after a Config keep their offsets.
+    uint16_t nbits;        // 1 .. min(255, 32 * swords)
+    uint16_t swords;       // 32-bit words per scalar: 1, 2, 4 or 8
 };
 
-// digits per scalar, D = ceil(256 / c) (equal to nwins without a table)
-HD uint32_t digit_count(const Config& cfg) { return (256 + cfg.wbits - 1) / cfg.wbits; }
+// digits per scalar, D = ceil((nbits + 1) / c) (equal to nwins without a table): the top digit never
+// carries out of the last window; ceil(256 / c) for 255-bit scalars
+HD uint32_t digits_for(uint32_t nbits, uint32_t wbits) { return (nbits + wbits) / wbits; }
+HD uint32_t digit_count(const Config& cfg) { return digits_for(cfg.nbits, cfg.wbits); }
 // entries per bucket-set row of `staging` / `sorted`: every copy of every point of the slice
 // (a 32-bit product: a table keeps copies * points < 2^31, the bucket entry's index range)
 HD size_t row_stride(const Config& cfg) { return cfg.copies * cfg.npoints; }
@@ -67,31 +74,46 @@ HD uint32_t atomic_inc(uint32_t* p, uint32_t v = 1)
 #endif
 }
 
-// 256-bit little-endian scalar -> signed digits d_w in (-2^(c-1), 2^(c-1)], sum d_w 2^(cw) = s.
+// little-endian scalar of SW 32-bit words -> signed digits d_w in (-2^(c-1), 2^(c-1)], sum d_w 2^(cw) = s.
+// The scalar is read with one load of its width (32, 64 or 128 bits; two 128-bit loads for 8 words).
+template<uint32_t SW>
 struct Digits {
-    uint32_t s[8];
+    uint32_t s[SW];
     uint32_t carry;
-    HD explicit Digits(const uint32_t* p) : carry(0)
+    HD Digits(const uint32_t* p, uint32_t nbits) : carry(0)
     {
 #if defined(__CUDA_ARCH__)
-        uint4 a = reinterpret_cast<const uint4*>(p)[0], b = reinterpret_cast<const uint4*>(p)[1];
-        s[0] = a.x; s[1] = a.y; s[2] = a.z; s[3] = a.w;
-        s[4] = b.x; s[5] = b.y; s[6] = b.z; s[7] = b.w;
+        if constexpr (SW == 1) {
+            s[0] = *p;
+        } else if constexpr (SW == 2) {
+            const uint2 a = *reinterpret_cast<const uint2*>(p);
+            s[0] = a.x; s[1] = a.y;
+        } else {
+#pragma unroll
+            for (uint32_t k = 0; k < SW / 4; k++) {
+                const uint4 a = reinterpret_cast<const uint4*>(p)[k];
+                s[4 * k] = a.x; s[4 * k + 1] = a.y; s[4 * k + 2] = a.z; s[4 * k + 3] = a.w;
+            }
+        }
 #else
-        for (int i = 0; i < 8; i++) s[i] = p[i];
+        for (uint32_t k = 0; k < SW; k++) s[k] = p[k];
 #endif
-        // Bit 255 is ignored, as the reference ignores every bit from `nbits` up
-        // (msm/pippenger.cuh:33-70, nbits = 255 or less for all supported scalar fields): with it
-        // cleared the top window can never carry out, also when the window width divides 256, so
-        // un-reduced inputs give a deterministic result instead of one that depends on npoints.
-        s[7] &= 0x7fffffffu;
+        // Bits from nbits up are ignored, as the reference ignores every bit from its `nbits` up
+        // (msm/pippenger.cuh:33-70; 255 for the 32-byte entries): with them cleared the top window
+        // can never carry out, also when the window width divides nbits + 1, so un-reduced inputs
+        // give a deterministic result instead of one that depends on npoints.
+#pragma unroll
+        for (uint32_t k = 0; k < SW; k++) {
+            if (32 * k >= nbits) s[k] = 0;
+            else if (nbits - 32 * k < 32) s[k] &= (1u << (nbits - 32 * k)) - 1;
+        }
     }
     // windows must be requested in order w = 0, 1, ...; returns bucket (|d|-1) and sign,
     // or false for a zero digit
     HD bool next(uint32_t w, uint32_t c, uint32_t& bucket, uint32_t& neg)
     {
         uint32_t off = w * c, i = off >> 5, sh = off & 31;
-        uint32_t lo = i < 8 ? s[i] : 0, hi = i + 1 < 8 ? s[i + 1] : 0;
+        uint32_t lo = i < SW ? s[i] : 0, hi = i + 1 < SW ? s[i + 1] : 0;
         uint32_t raw = sh ? (lo >> sh) | (hi << (32 - sh)) : lo;
         raw = (c < 32 ? raw & ((1u << c) - 1) : raw) + carry;
         const uint32_t half = 1u << (c - 1);
@@ -108,6 +130,19 @@ struct Digits {
     }
 };
 
+// fn(Digits<swords>&) for scalar i of a scalar array in the format of cfg (host-side bodies: the
+// device kernels are instantiated per width instead)
+template<class Fn>
+HD void with_digits(const Config& cfg, const uint32_t* scalars, uint32_t i, Fn fn)
+{
+    switch (cfg.swords) {
+    case 1: { Digits<1> d(scalars + (size_t)i, cfg.nbits); fn(d); break; }
+    case 2: { Digits<2> d(scalars + 2 * (size_t)i, cfg.nbits); fn(d); break; }
+    case 4: { Digits<4> d(scalars + 4 * (size_t)i, cfg.nbits); fn(d); break; }
+    default: { Digits<8> d(scalars + 8 * (size_t)i, cfg.nbits); fn(d); break; }
+    }
+}
+
 // ---- direct sort: one counter and one cursor per (window, bucket) ----------------------------
 // The plain form of the sort below: count every entry into its bucket, exclusive prefix per window,
 // place every entry at its bucket's cursor.  It produces the same counts, offsets and bucket lists
@@ -116,28 +151,30 @@ struct Digits {
 // random 4-byte stores keep more partly written lines open than L2 holds.
 HD void count_body(const Config& cfg, const uint32_t* scalars, uint32_t* counts, uint32_t i)
 {
-    Digits d(scalars + 8 * (size_t)i);
-    const uint32_t nd = digit_count(cfg);
-    for (uint32_t w = 0; w < nd; w++) {
-        uint32_t b, neg, entry;
-        if (d.next(w, cfg.wbits, b, neg))
-            atomic_inc(&counts[((size_t)digit_slot(cfg, w, i, neg, entry) << cfg.lg_nb) + b]);
-    }
+    with_digits(cfg, scalars, i, [&](auto& d) {
+        const uint32_t nd = digit_count(cfg);
+        for (uint32_t w = 0; w < nd; w++) {
+            uint32_t b, neg, entry;
+            if (d.next(w, cfg.wbits, b, neg))
+                atomic_inc(&counts[((size_t)digit_slot(cfg, w, i, neg, entry) << cfg.lg_nb) + b]);
+        }
+    });
 }
 
 // digits [w0, w1) only: digits below w0 are still walked for their carry
 HD void scatter_body(const Config& cfg, const uint32_t* scalars, uint32_t* cursor,
                      uint32_t* sorted, uint32_t i, uint32_t w0, uint32_t w1)
 {
-    Digits d(scalars + 8 * (size_t)i);
-    for (uint32_t w = 0; w < w1; w++) {
-        uint32_t b, neg, entry;
-        if (d.next(w, cfg.wbits, b, neg) && w >= w0) {
-            const uint32_t v = digit_slot(cfg, w, i, neg, entry);
-            uint32_t pos = atomic_inc(&cursor[((size_t)v << cfg.lg_nb) + b]);
-            sorted[(size_t)v * row_stride(cfg) + pos] = entry;
+    with_digits(cfg, scalars, i, [&](auto& d) {
+        for (uint32_t w = 0; w < w1; w++) {
+            uint32_t b, neg, entry;
+            if (d.next(w, cfg.wbits, b, neg) && w >= w0) {
+                const uint32_t v = digit_slot(cfg, w, i, neg, entry);
+                uint32_t pos = atomic_inc(&cursor[((size_t)v << cfg.lg_nb) + b]);
+                sorted[(size_t)v * row_stride(cfg) + pos] = entry;
+            }
         }
-    }
+    });
 }
 
 // ---- sort: (window, bucket) lists of point indices -----------------------------------------
@@ -153,11 +190,12 @@ HD void scatter_body(const Config& cfg, const uint32_t* scalars, uint32_t* curso
 constexpr uint32_t SORT_SMAX = 12;      // a bin spans at most 2^12 buckets (its shared histogram)
 constexpr uint32_t SORT_LG_FILL = 13;   // bins hold about 2^13 entries of a uniform window
 
-// bits of the top window's digit magnitude: bit 255 is ignored, so the window holds bits
-// (W-1)c..254 plus the carry and its buckets are < 2^(255 - (W-1)c) (at most 2^(c-1))
+// bits of the top window's digit magnitude: bits from nbits up are ignored, so the window holds bits
+// (W-1)c..nbits-1 plus the carry and its buckets are < 2^(nbits - (W-1)c) (at most 2^(c-1); 2^0 when
+// c divides nbits and the window holds only the carry)
 HD uint32_t top_window_bits(const Config& cfg)
 {
-    const uint32_t e = 255 - (cfg.nwins - 1) * cfg.wbits;
+    const uint32_t e = cfg.nbits - (cfg.nwins - 1) * cfg.wbits;
     return e < cfg.lg_nb ? e : cfg.lg_nb;
 }
 // with a table the thin top digit shares its bucket set with full-width digits: every set is full
@@ -199,12 +237,12 @@ HD bool last_bin(const Config& cfg, uint32_t lg_bins, uint32_t w, uint32_t bin)
 // every digit of point i in order: fn(set, nonzero, bin (global), bucket, entry), with set and entry
 // from digit_slot (without a table: set = digit index, entry = i | sign << 31).  Digits >= w_end are
 // not visited.  `valid` false: fn sees only zero digits (the tail lanes of a warp that must still
-// take part in its collective operations).
-template<class Fn>
+// take part in its collective operations).  SW: cfg.swords, the scalar width the kernel is built for.
+template<uint32_t SW = 8, class Fn>
 HD void for_each_digit(const Config& cfg, uint32_t lg_bins, const uint32_t* scalars, uint32_t i, bool valid,
                        uint32_t w_end, Fn fn)
 {
-    Digits d(scalars + 8 * (size_t)(valid ? i : 0));
+    Digits<SW> d(scalars + SW * (size_t)(valid ? i : 0), cfg.nbits);
     for (uint32_t w = 0; w < w_end; w++) {
         uint32_t b, neg, entry;
         const bool nz = d.next(w, cfg.wbits, b, neg) && valid;
@@ -400,19 +438,20 @@ HD void finish_body(const Config& cfg, const uint32_t* winR, uint32_t* out_jacob
 // window width minimising the measured cost model (fitted on an earlier GPU; not refitted for H100):
 //   per (point, window): 1 mixed add + ~0.11 for count/scatter;  per bucket: ~5.5 mixed-add
 //   equivalents for the two full adds of the running sum
-inline uint32_t choose_wbits(size_t npoints)
+// over the W = ceil((nbits + 1) / c) windows of nbits-bit scalars (255: the 32-byte entries)
+inline uint32_t choose_wbits(size_t npoints, uint32_t nbits)
 {
     uint32_t best = 4;
     double best_cost = 1e300;
     for (uint32_t c = 4; c <= 22; c++) {
-        uint32_t nwins = (256 + c - 1) / c;
+        uint32_t nwins = digits_for(nbits, c);
         double cost = (double)nwins * (1.11 * (double)npoints + 5.5 * (double)(1u << (c - 1)));
         // a top window of only a few bits puts npoints / 2^e entries into each of its 2^e buckets: the
         // count / scatter atomics collide on them and they go through the heavy-bucket path; at 2^23
         // points c = 16 (no thin window) measured faster than the c = 18 this model ranks first
         // without the term (on the GPU the model was fitted on).  Left alone below 2^22 points,
         // where the table was tuned without it.
-        const uint32_t e = 256 - (nwins - 1) * c;                 // bits of the top window
+        const uint32_t e = nbits + 1 - (nwins - 1) * c;           // bits of the top window
         if (npoints >= ((size_t)1 << 22) && e <= 10 && (npoints >> e) > 2048) cost += 1.25 * (double)npoints;
         if (cost < best_cost) { best_cost = cost; best = c; }
     }
@@ -422,6 +461,7 @@ inline uint32_t choose_wbits(size_t npoints)
     }
     return best;
 }
+inline uint32_t choose_wbits(size_t npoints) { return choose_wbits(npoints, 255); }
 
 // a bucket is "heavy" when one lane folding it alone would take longer than that lane's fair
 // share of the whole job (57k lanes: the resident lane count the constant was chosen for; an
@@ -438,38 +478,51 @@ inline void set_heavy(Config& cfg, uint64_t entries)
     if (const char* env = getenv("SPPARK_B200_MSM_HEAVY")) cfg.heavy = (uint32_t)atoi(env);
 }
 
-inline Config make_config(size_t npoints)
+// the geometry of an MSM over npoints scalars of scalar_bytes bytes whose bits from nbits up are ignored
+inline Config make_config(size_t npoints, uint32_t nbits, uint32_t scalar_bytes)
 {
     Config cfg;
-    cfg.wbits = choose_wbits(npoints);
-    cfg.nwins = (256 + cfg.wbits - 1) / cfg.wbits;
+    cfg.wbits = choose_wbits(npoints, nbits);
+    cfg.nwins = digits_for(nbits, cfg.wbits);
     cfg.lg_nb = cfg.wbits - 1;
     cfg.npoints = (uint32_t)npoints;
     cfg.merge = 0;
     cfg.copies = 1;
     cfg.copy_stride = (uint32_t)npoints;
+    cfg.nbits = (uint16_t)nbits;
+    cfg.swords = (uint16_t)(scalar_bytes / 4);
     set_heavy(cfg, (uint64_t)cfg.nwins * npoints);
     return cfg;
 }
+inline Config make_config(size_t npoints) { return make_config(npoints, 255, 32); }
 
 // ---- precomputed tables ---------------------------------------------------------------------
 // The geometry of a table of width c built for at most `copies` copies: V = ceil(D / K) bucket sets,
 // K_used = ceil(D / V) <= K copies stored (more would add no set), for an MSM over n points of a
 // table whose copies are `stride` points apart.  The heavy threshold follows the D * n entries.
-inline Config config_for_table(size_t n, uint32_t wbits, uint32_t copies, size_t stride)
+// With nbits-bit scalars only the digits w < D_b = ceil((nbits + 1) / c) are walked: the sets stay
+// the table's V and copies 0 .. ceil(D_b / V) - 1 are read; when D_b <= V only copy 0 is, and the
+// geometry is the plain one of width c (D_b sets, its thin top window included).
+inline Config config_for_table(size_t n, uint32_t wbits, uint32_t copies, size_t stride, uint32_t nbits,
+                               uint32_t scalar_bytes)
 {
     Config cfg;
-    const uint32_t D = (256 + wbits - 1) / wbits, K = std::max(1u, std::min(copies, D));
+    const uint32_t D = digits_for(255, wbits), K = std::max(1u, std::min(copies, D)), V = (D + K - 1) / K;
+    const uint32_t Db = digits_for(nbits, wbits);
     cfg.wbits = wbits;
-    cfg.nwins = (D + K - 1) / K;
+    cfg.nwins = std::min(V, Db);
     cfg.lg_nb = wbits - 1;
     cfg.npoints = (uint32_t)n;
     cfg.merge = 0;
-    cfg.copies = (D + cfg.nwins - 1) / cfg.nwins;
+    cfg.copies = (Db + cfg.nwins - 1) / cfg.nwins;
     cfg.copy_stride = (uint32_t)stride;
-    set_heavy(cfg, (uint64_t)D * n);
+    cfg.nbits = (uint16_t)nbits;
+    cfg.swords = (uint16_t)(scalar_bytes / 4);
+    set_heavy(cfg, (uint64_t)Db * n);
     return cfg;
 }
+inline Config config_for_table(size_t n, uint32_t wbits, uint32_t copies, size_t stride)
+{   return config_for_table(n, wbits, copies, stride, 255, 32);   }
 
 // N points, at most K copies: make_config for K = 1; otherwise the width c in [4, 24] minimising the
 // window cost model of choose_wbits re-scored for the table, 1.11 D N + 5.5 V 2^(c-1) (the mixed
@@ -480,7 +533,7 @@ inline Config make_config_precomputed(size_t npoints, uint32_t copies)
     uint32_t best = 4;
     double best_cost = 1e300;
     for (uint32_t c = 4; c <= 24; c++) {
-        const uint32_t D = (256 + c - 1) / c, V = (D + copies - 1) / copies;
+        const uint32_t D = digits_for(255, c), V = (D + copies - 1) / copies;
         const double cost = 1.11 * (double)D * (double)npoints + 5.5 * (double)V * (double)(1u << (c - 1));
         if (cost < best_cost) { best_cost = cost; best = c; }
     }

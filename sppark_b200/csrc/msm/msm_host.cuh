@@ -44,10 +44,12 @@ typedef void (*unmont_fn)(uint32_t*, size_t, cudaStream_t);
 // msm/pippenger.cuh:377-390,582-601): only the scalars cross PCIe, sliced the same way.
 // `table` (with `resident`): the rows are a precomputed table of that width and copy count, whose
 // copies lie table->copy_stride rows apart; slice k's points start at row `first` of every copy.
+// scalar_bytes / nbits: the scalar format (msm_core.cuh Config); each slice uploads n * scalar_bytes.
 template<class F>
 RustError msm_host(void* out, const void* points, size_t npoints, const void* scalars,
                    size_t stride, bool has_flag, unmont_fn unmont = nullptr,
-                   const uint32_t* resident = nullptr, const msm::Config* table = nullptr)
+                   const uint32_t* resident = nullptr, const msm::Config* table = nullptr,
+                   uint32_t scalar_bytes = 32, uint32_t nbits = 255)
 {
     constexpr size_t PB = 2 * F::N * 4, JB = 3 * F::N * 4;
     try {
@@ -112,7 +114,8 @@ RustError msm_host(void* out, const void* points, size_t npoints, const void* sc
         };
 
         dev_ptr_t<uint32_t> d_out(JB / 4, compute);
-        dev_ptr_t<uint32_t> d_points(resident ? 1 : nbuf * slice_n * (PB / 4), compute), d_scalars(nbuf * slice_n * 8, compute);
+        const size_t SW = scalar_bytes / 4;                        // 32-bit words per scalar
+        dev_ptr_t<uint32_t> d_points(resident ? 1 : nbuf * slice_n * (PB / 4), compute), d_scalars(nbuf * slice_n * SW, compute);
         dev_ptr_t<uint8_t> d_raw(packed ? 1 : nbuf * slice_n * stride, compute);
         event_t copied[2], consumed[2], ready;
         ready.record(compute);                                    // buffers exist
@@ -127,16 +130,17 @@ RustError msm_host(void* out, const void* points, size_t npoints, const void* sc
         } drain{compute, copy};
 
         msm::msm_t<F> m(gpu);
-        auto job = table ? m.begin(msm::config_for_table(npoints, table->wbits, table->copies, table->copy_stride),
+        auto job = table ? m.begin(msm::config_for_table(npoints, table->wbits, table->copies, table->copy_stride,
+                                                         nbits, scalar_bytes),
                                    slice_n, compute)
-                         : m.begin(npoints, slice_n, compute);
+                         : m.begin(npoints, slice_n, compute, nbits, scalar_bytes);
         size_t first = 0;
         for (size_t k = 0; k < nslices; first += sched[k], k++) {
             const size_t b = k & (nbuf - 1), n = sched[k];
             const uint32_t* dp = resident ? resident + first * (PB / 4) : d_points + b * slice_n * (PB / 4);
-            uint32_t* ds = d_scalars + b * slice_n * 8;
+            uint32_t* ds = d_scalars + b * slice_n * SW;
             if (k >= nbuf) consumed[b].wait(copy);                                // buffer free again
-            upload(ds, (const uint8_t*)scalars + first * 32, n * 32);
+            upload(ds, (const uint8_t*)scalars + first * scalar_bytes, n * scalar_bytes);
             if (resident) {
             } else if (packed) {
                 upload(d_points + b * slice_n * (PB / 4), (const uint8_t*)points + first * PB, n * PB);
@@ -236,20 +240,25 @@ RustError msm_preload(const void* points, size_t npoints, size_t stride, bool ha
 }
 
 // MSM of host scalars against the first npoints rows of a msm_preload buffer; wbits / copies /
-// copy_stride: the table it holds (copies = 1: plain rows, the window width follows npoints)
+// copy_stride: the table it holds (copies = 1: plain rows, the window width follows npoints and the
+// scalar format)
 template<class F, class Fr>
 RustError msm_resident(void* out, const void* d_points, size_t npoints, const void* scalars, bool mont,
-                       uint32_t wbits, uint32_t copies, size_t copy_stride)
+                       uint32_t wbits, uint32_t copies, size_t copy_stride, uint32_t scalar_bytes = 32,
+                       uint32_t nbits = 255)
 {
     const unmont_fn unmont = mont ? scalars_from_mont<Fr> : nullptr;
     if (copies <= 1)
-        return msm_host<F>(out, nullptr, npoints, scalars, 0, false, unmont, (const uint32_t*)d_points);
+        return msm_host<F>(out, nullptr, npoints, scalars, 0, false, unmont, (const uint32_t*)d_points, nullptr,
+                           scalar_bytes, nbits);
     const msm::Config table = msm::config_for_table(copy_stride, wbits, copies, copy_stride);
-    return msm_host<F>(out, nullptr, npoints, scalars, 0, false, unmont, (const uint32_t*)d_points, &table);
+    return msm_host<F>(out, nullptr, npoints, scalars, 0, false, unmont, (const uint32_t*)d_points, &table,
+                       scalar_bytes, nbits);
 }
 
 template<class F>
-RustError msm_dev(void* out, const void* d_points, size_t npoints, const void* d_scalars, void* stream)
+RustError msm_dev(void* out, const void* d_points, size_t npoints, const void* d_scalars, void* stream,
+                  uint32_t scalar_bytes = 32, uint32_t nbits = 255)
 {
     constexpr size_t JB = 3 * F::N * 4;
     try {
@@ -258,7 +267,7 @@ RustError msm_dev(void* out, const void* d_points, size_t npoints, const void* d
         const stream_t borrowed(s);
         dev_ptr_t<uint32_t> d_out(JB / 4, borrowed);           // released on every exit path
         msm::msm_t<F> m(gpu);
-        m.invoke_dev(d_out, (const uint32_t*)d_points, npoints, (const uint32_t*)d_scalars, s);
+        m.invoke_dev(d_out, (const uint32_t*)d_points, npoints, (const uint32_t*)d_scalars, s, nbits, scalar_bytes);
         CUDA_OK(cudaMemcpyAsync(out, d_out, JB, cudaMemcpyDeviceToHost, s));
         CUDA_OK(cudaStreamSynchronize(s));
     } catch (const cuda_error& e) {

@@ -56,16 +56,67 @@ def multi_scalar_mult_fp2_arkworks(points, scalars):
     return out
 
 
-def msm(curve, points, scalars, mont=False):
+def _scalar_bytes(scalars, u64, u32):
+    """bytes per scalar from the array's shape and dtype: (n, 4) 64-bit words 32, (n, 2) 16, (n,) 64-bit 8,
+    (n,) 32-bit 4; None for any other array"""
+    if scalars.ndim == 2 and scalars.dtype == u64 and scalars.shape[1] in (2, 4):
+        return 8 * scalars.shape[1]
+    if scalars.ndim == 1 and scalars.dtype in (u64, u32):
+        return 8 if scalars.dtype == u64 else 4
+    return None
+
+
+def _scalar_format(sbytes, mont, nbits):
+    """(scalar_bytes, nbits) of a small-scalar call, or None for today's 32-byte call"""
+    if sbytes == 32 and nbits is None:
+        return None
+    if mont:
+        raise ValueError("mont=True takes (n, 4) scalars without nbits")
+    if nbits is None:
+        nbits = min(255, 8 * sbytes)
+    if not 1 <= nbits <= min(255, 8 * sbytes):
+        raise ValueError(f"nbits must be in [1, {min(255, 8 * sbytes)}] for {sbytes}-byte scalars")
+    return sbytes, int(nbits)
+
+
+def _host_format(scalars, mont, nbits):
+    sbytes = _scalar_bytes(scalars, np.uint64, np.uint32)
+    if sbytes is None:
+        raise TypeError("scalars must be (n, 4) or (n, 2) uint64, (n,) uint64 or (n,) uint32")
+    return _scalar_format(sbytes, mont, nbits)
+
+
+def _check_compact(points, scalars):
+    if points.shape[0] != scalars.shape[0]:
+        raise ValueError("length mismatch")
+    if not (points.flags["C_CONTIGUOUS"] and scalars.flags["C_CONTIGUOUS"]):
+        raise TypeError("points and scalars must be C-contiguous")
+    if points.dtype != np.uint64:
+        raise TypeError("points must be a uint64 limb array")
+
+
+def msm(curve, points, scalars, mont=False, nbits=None):
     """Any supported curve; host arrays of packed affine points (n, 2*limbs) or rows with an
     infinity-flag word appended (n, 2*limbs + 1).  mont=True: the scalars are Montgomery residues
-    (the `mont` flag of the reference's C++ template, msm/pippenger.cuh:730-733)."""
-    _check(points, scalars)
+    (the `mont` flag of the reference's C++ template, msm/pippenger.cuh:730-733).
+
+    Small scalars: the scalar width follows the array, (n, 4) uint64 32 bytes, (n, 2) uint64 16,
+    (n,) uint64 8, (n,) uint32 4; bits from `nbits` up are ignored (default min(255, 8 * width)).
+    Fewer bits mean fewer windows and fewer bytes over PCIe (DESIGN.md section 5c)."""
+    fmt = _host_format(scalars, mont, nbits)
+    if fmt is None:
+        _check(points, scalars)
+    else:
+        _check_compact(points, scalars)
     nl = _LIMBS[curve]
     assert points.shape[1] in (2 * nl, 2 * nl + 1)
     out = np.zeros(3 * nl, dtype=np.uint64)
-    err = _lib.lib().sppark_b200_msm_ex(curve, out.ctypes.data, points.ctypes.data, points.shape[0],
-                                        scalars.ctypes.data, points.strides[0], int(mont))
+    if fmt is None:
+        err = _lib.lib().sppark_b200_msm_ex(curve, out.ctypes.data, points.ctypes.data, points.shape[0],
+                                            scalars.ctypes.data, points.strides[0], int(mont))
+    else:
+        err = _lib.lib().sppark_b200_msm_bits(curve, out.ctypes.data, points.ctypes.data, points.shape[0],
+                                              scalars.ctypes.data, points.strides[0], *fmt)
     _lib.check(err)
     return out
 
@@ -94,12 +145,22 @@ class MsmContext:
                                                                     C.byref(self._h))
         _lib.check(err)
 
-    def invoke(self, scalars, mont=False):
-        if scalars.dtype != np.uint64 or scalars.ndim != 2 or scalars.shape[1] != 4 or not scalars.flags["C_CONTIGUOUS"]:
+    def invoke(self, scalars, mont=False, nbits=None):
+        """scalars: (n, 4) uint64, or a small-scalar array with an optional bit bound as for msm()"""
+        fmt = _host_format(scalars, mont, nbits) if scalars.dtype in (np.uint64, np.uint32) else None
+        if fmt is None and (scalars.dtype != np.uint64 or scalars.ndim != 2 or scalars.shape[1] != 4
+                            or not scalars.flags["C_CONTIGUOUS"]):
             raise TypeError("scalars must be a C-contiguous (n, 4) uint64 array")
+        if fmt is not None and not scalars.flags["C_CONTIGUOUS"]:
+            raise TypeError("scalars must be C-contiguous")
         out = np.zeros(3 * _LIMBS[self.curve], dtype=np.uint64)
-        _lib.check(_lib.lib().sppark_b200_msm_ctx_invoke(self._h, out.ctypes.data, scalars.ctypes.data,
-                                                         scalars.shape[0], int(mont)))
+        if fmt is None:
+            err = _lib.lib().sppark_b200_msm_ctx_invoke(self._h, out.ctypes.data, scalars.ctypes.data,
+                                                        scalars.shape[0], int(mont))
+        else:
+            err = _lib.lib().sppark_b200_msm_ctx_invoke_bits(self._h, out.ctypes.data, scalars.ctypes.data,
+                                                             scalars.shape[0], *fmt)
+        _lib.check(err)
         return out
 
     def close(self):
@@ -114,19 +175,30 @@ class MsmContext:
             pass
 
 
-def msm_dev(curve, d_points, d_scalars, npoints=None, stream=None):
+def msm_dev(curve, d_points, d_scalars, npoints=None, stream=None, nbits=None):
     """msm_t::invoke with device-resident inputs (msm/pippenger.cuh:582-601): torch CUDA tensors
     of packed affine points / 32-byte scalars; synchronises the stream and returns the Jacobian
-    result as a host array."""
+    result as a host array.
+
+    Small scalars as for msm(), with int64 / int32 tensors: (n, 2) int64 16 bytes, (n,) int64 8,
+    (n,) int32 4; bits from `nbits` up are ignored.  Any other tensor holds 32-byte scalars."""
     import torch
     nl = _LIMBS[curve]
     assert d_points.is_cuda and d_scalars.is_cuda and d_points.is_contiguous() and d_scalars.is_contiguous()
-    n = npoints if npoints is not None else d_scalars.numel() * d_scalars.element_size() // 32
+    sbytes = _scalar_bytes(d_scalars, torch.int64, torch.int32)
+    if sbytes is None and nbits is not None:
+        raise TypeError("a bit bound takes (n, 4) or (n, 2) int64, (n,) int64 or (n,) int32 scalars")
+    fmt = _scalar_format(sbytes or 32, False, nbits)
+    n = npoints if npoints is not None else d_scalars.numel() * d_scalars.element_size() // (fmt[0] if fmt else 32)
     out = np.zeros(3 * nl, dtype=np.uint64)
     with torch.cuda.device(d_points.device):
         s = stream if stream is not None else torch.cuda.current_stream().cuda_stream
-        err = _lib.lib().sppark_b200_msm_dev(curve, out.ctypes.data, d_points.data_ptr(), n,
-                                             d_scalars.data_ptr(), s)
+        if fmt is None:
+            err = _lib.lib().sppark_b200_msm_dev(curve, out.ctypes.data, d_points.data_ptr(), n,
+                                                 d_scalars.data_ptr(), s)
+        else:
+            err = _lib.lib().sppark_b200_msm_dev_bits(curve, out.ctypes.data, d_points.data_ptr(), n,
+                                                      d_scalars.data_ptr(), fmt[0], fmt[1], s)
     _lib.check(err)
     return out
 
