@@ -21,7 +21,11 @@ NVCC_FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "
 
 
 def _sources():
-    return [os.path.join(CSRC, s) for s in SOURCES if os.path.exists(os.path.join(CSRC, s))]
+    paths = [os.path.join(CSRC, s) for s in SOURCES]
+    missing = [p for p in paths if not os.path.exists(p)]
+    if missing:
+        raise FileNotFoundError("missing sources: " + ", ".join(missing))
+    return paths
 
 
 def _newest_input():
@@ -68,7 +72,10 @@ def build(force=False, verbose=False):
     for p, cmd in procs:
         if p.wait() != 0:
             raise RuntimeError("nvcc failed: " + " ".join(cmd))
-    subprocess.check_call(["nvcc", "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a"])
+    # --no-undefined: a symbol that is declared but that no object defines fails the link, not the
+    # library's load
+    subprocess.check_call(["nvcc", "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a",
+                           "-Xlinker", "--no-undefined"])
     return LIB
 
 

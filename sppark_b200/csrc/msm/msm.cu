@@ -1,49 +1,40 @@
-// Curve dispatch for the extended MSM entry points (include/sppark_b200.h).
+// Curve dispatch for the MSM entry points, drop-in and extended (include/sppark_b200.h).
 #include "../util/gpu.cuh"
+#include "curve_ops.cuh"
 #include <cstring>
 #include <thread>
 #include <vector>
 
-// one row per curve id (SPPARK_CURVE_*): the six entry points its translation unit defines
-// (msm_bls12_381.cu, msm_pasta.cu, msm_bn254_bls12_377.cu, msm_*_g2.cu) and its packed layouts.
-// The MSM entries end in the scalar format (scalar_bytes, nbits): 32, 255 for 32-byte scalars.
-#define CURVE_DECLS(name)                                                                          \
-    RustError msm_host_##name(void*, const void*, size_t, const void*, size_t, bool, bool,         \
-                              uint32_t, uint32_t);                                                 \
-    RustError msm_dev_##name(void*, const void*, size_t, const void*, void*, uint32_t, uint32_t);  \
-    RustError gen_points_##name(void*, size_t, void*);                                             \
-    RustError combine_##name(void*, const void*, size_t);                                          \
-    RustError msm_preload_##name(const void*, size_t, size_t, bool, void**, uint32_t*, uint32_t*); \
-    RustError msm_resident_##name(void*, const void*, size_t, const void*, bool, uint32_t, uint32_t, size_t, \
-                                  uint32_t, uint32_t);
-CURVE_DECLS(bls12_381) CURVE_DECLS(pallas) CURVE_DECLS(vesta) CURVE_DECLS(bls12_381_g2)
-CURVE_DECLS(bn254) CURVE_DECLS(bls12_377) CURVE_DECLS(bn254_g2) CURVE_DECLS(bls12_377_g2)
-
-struct curve_ops {
-    RustError (*host)(void*, const void*, size_t, const void*, size_t, bool, bool, uint32_t, uint32_t);
-    RustError (*dev)(void*, const void*, size_t, const void*, void*, uint32_t, uint32_t);
-    RustError (*gen)(void*, size_t, void*);
-    RustError (*combine)(void*, const void*, size_t);
-    RustError (*preload)(const void*, size_t, size_t, bool, void**, uint32_t*, uint32_t*);
-    RustError (*resident)(void*, const void*, size_t, const void*, bool, uint32_t, uint32_t, size_t, uint32_t, uint32_t);
-    size_t affine_bytes, jacobian_bytes;        // packed {X, Y} and {X, Y, Z}
-};
-#define CURVE_ROW(name, affine, jac)                                                               \
-    {msm_host_##name, msm_dev_##name, gen_points_##name, combine_##name, msm_preload_##name,       \
-     msm_resident_##name, affine, jac}
-static const curve_ops CURVES[] = {
-    CURVE_ROW(bls12_381, 96, 144),        // SPPARK_CURVE_BLS12_381_G1
-    CURVE_ROW(pallas, 64, 96),            // SPPARK_CURVE_PALLAS
-    CURVE_ROW(vesta, 64, 96),             // SPPARK_CURVE_VESTA
-    CURVE_ROW(bls12_381_g2, 192, 288),    // SPPARK_CURVE_BLS12_381_G2
-    CURVE_ROW(bn254, 64, 96),             // SPPARK_CURVE_BN254_G1
-    CURVE_ROW(bls12_377, 96, 144),        // SPPARK_CURVE_BLS12_377_G1
-    CURVE_ROW(bn254_g2, 128, 192),        // SPPARK_CURVE_BN254_G2
-    CURVE_ROW(bls12_377_g2, 192, 288),    // SPPARK_CURVE_BLS12_377_G2
+// one row per curve id (curve_ops.cuh)
+static const curve_ops* const CURVES[] = {
+    &curve_bls12_381,       // SPPARK_CURVE_BLS12_381_G1
+    &curve_pallas,          // SPPARK_CURVE_PALLAS
+    &curve_vesta,           // SPPARK_CURVE_VESTA
+    &curve_bls12_381_g2,    // SPPARK_CURVE_BLS12_381_G2
+    &curve_bn254,           // SPPARK_CURVE_BN254_G1
+    &curve_bls12_377,       // SPPARK_CURVE_BLS12_377_G1
+    &curve_bn254_g2,        // SPPARK_CURVE_BN254_G2
+    &curve_bls12_377_g2,    // SPPARK_CURVE_BLS12_377_G2
 };
 static_assert(sizeof(CURVES) / sizeof(CURVES[0]) == SPPARK_CURVE_BLS12_377_G2 + 1, "one row per curve id");
 static const curve_ops* curve_of(int curve)
-{   return curve < 0 || curve > SPPARK_CURVE_BLS12_377_G2 ? nullptr : &CURVES[curve];   }
+{   return curve < 0 || curve > SPPARK_CURVE_BLS12_377_G2 ? nullptr : CURVES[curve];   }
+
+// the drop-in entry points of poc/msm-cuda: BLS12-381 host points, 32-byte scalars
+//   mult_pippenger           poc/msm-cuda/cuda/pippenger.cu:20-25       G1, packed {X, Y} rows
+//   mult_pippenger_inf       poc/msm-cuda/cuda/pippenger_inf.cu:28-34   G1, rows of ffi_affine_sz bytes
+//   mult_pippenger_fp2_inf   poc/msm-cuda/cuda/pippenger_inf.cu:36-43   G2, rows of ffi_affine_sz bytes
+// The _inf rows always carry the infinity flag after Y, so a stride with no room for it is refused.
+extern "C" RustError mult_pippenger(void* out, const void* points, size_t npoints, const void* scalars)
+{   return curve_bls12_381.host(out, points, npoints, scalars, 96, false, false, 32, 255);   }
+
+extern "C" RustError mult_pippenger_inf(void* out, const void* points, size_t npoints,
+                                        const void* scalars, size_t ffi_affine_sz)
+{   return curve_bls12_381.host(out, points, npoints, scalars, ffi_affine_sz, true, false, 32, 255);   }
+
+extern "C" RustError mult_pippenger_fp2_inf(void* out, const void* points, size_t npoints,
+                                            const void* scalars, size_t ffi_affine_sz)
+{   return curve_bls12_381_g2.host(out, points, npoints, scalars, ffi_affine_sz, true, false, 32, 255);   }
 
 extern "C" RustError sppark_b200_generate_points_dev(int curve, void* d_out, size_t n, void* stream)
 {
@@ -70,17 +61,21 @@ static RustError msm_any(int curve, void* out, const void* points, size_t npoint
                    ffi_affine_sz > c->affine_bytes, mont, scalar_bytes, nbits);
 }
 
-// the scalar format of the _bits entries: 4, 8, 16 or 32 bytes, 1 <= nbits <= min(255, 8 * bytes)
-static bool scalar_format_ok(uint32_t scalar_bytes, uint32_t nbits)
-{
-    const bool width = scalar_bytes == 4 || scalar_bytes == 8 || scalar_bytes == 16 || scalar_bytes == 32;
-    return width && nbits >= 1 && nbits <= 255 && nbits <= 8 * scalar_bytes;
-}
 // a refused call returns infinity, as a failed MSM does
-static RustError refuse(void* out, size_t jacobian_bytes, const char* msg)
+static RustError refuse(void* out, size_t jacobian_bytes, const std::string& msg)
 {
     if (out) memset(out, 0, jacobian_bytes);
     return rust_err(-(int)cudaErrorInvalidValue, msg);
+}
+// the scalar format of the _bits entries: 4, 8, 16 or 32 bytes, 1 <= nbits <= min(255, 8 * bytes);
+// code 0 when it is one
+static RustError check_scalar_format(const char* entry, const curve_ops* c, void* out, uint32_t scalar_bytes,
+                                     uint32_t nbits)
+{
+    const bool width = scalar_bytes == 4 || scalar_bytes == 8 || scalar_bytes == 16 || scalar_bytes == 32;
+    if (width && nbits >= 1 && nbits <= 255 && nbits <= 8 * scalar_bytes) return rust_ok();
+    return refuse(out, c->jacobian_bytes, std::string(entry) + ": scalar_bytes must be 4, 8, 16 or 32 and "
+                                                               "1 <= nbits <= min(255, 8 * scalar_bytes)");
 }
 
 extern "C" RustError sppark_b200_msm_bits(int curve, void* out, const void* points, size_t npoints,
@@ -89,9 +84,8 @@ extern "C" RustError sppark_b200_msm_bits(int curve, void* out, const void* poin
 {
     const curve_ops* c = curve_of(curve);
     if (c == nullptr) return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_msm_bits: unknown curve");
-    if (!scalar_format_ok(scalar_bytes, nbits))
-        return refuse(out, c->jacobian_bytes, "sppark_b200_msm_bits: scalar_bytes must be 4, 8, 16 or 32 and "
-                                              "1 <= nbits <= min(255, 8 * scalar_bytes)");
+    const RustError e = check_scalar_format("sppark_b200_msm_bits", c, out, scalar_bytes, nbits);
+    if (e.code != 0) return e;
     return msm_any(curve, out, points, npoints, scalars, ffi_affine_sz, false, scalar_bytes, nbits);
 }
 
@@ -117,9 +111,8 @@ extern "C" RustError sppark_b200_msm_dev_bits(int curve, void* out, const void* 
 {
     const curve_ops* c = curve_of(curve);
     if (c == nullptr) return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_msm_dev_bits: unknown curve");
-    if (!scalar_format_ok(scalar_bytes, nbits))
-        return refuse(out, c->jacobian_bytes, "sppark_b200_msm_dev_bits: scalar_bytes must be 4, 8, 16 or 32 and "
-                                              "1 <= nbits <= min(255, 8 * scalar_bytes)");
+    const RustError e = check_scalar_format("sppark_b200_msm_dev_bits", c, out, scalar_bytes, nbits);
+    if (e.code != 0) return e;
     if ((uintptr_t)d_scalars % (scalar_bytes < 16 ? scalar_bytes : 16) != 0)   // one aligned load per scalar
         return refuse(out, c->jacobian_bytes, "sppark_b200_msm_dev_bits: d_scalars must be aligned to "
                                               "min(scalar_bytes, 16) bytes");
@@ -231,33 +224,31 @@ extern "C" RustError sppark_b200_msm_ctx_create_precomputed(int curve, const voi
     return ctx_create(curve, points, npoints, ffi_affine_sz, copies, out);
 }
 
-extern "C" RustError sppark_b200_msm_ctx_invoke(sppark_b200_msm_ctx* ctx, void* out, const void* scalars,
-                                                size_t npoints, int scalars_mont)
+// the body of both invoke entries; a null context counts as one without points
+static RustError ctx_invoke(const char* entry, sppark_b200_msm_ctx* ctx, void* out, const void* scalars,
+                            size_t npoints, bool mont, uint32_t scalar_bytes, uint32_t nbits)
 {
     if (ctx == nullptr || npoints > ctx->npoints)
-        return rust_err(-(int)cudaErrorInvalidValue, "msm_ctx_invoke: more scalars than preloaded points");
+        return rust_err(-(int)cudaErrorInvalidValue, std::string(entry) + ": more scalars than preloaded points");
     int cur = 0;
     (void)cudaGetDevice(&cur);
-    if (cur != ctx->device) return rust_err(-(int)cudaErrorInvalidDevice, "msm_ctx_invoke: the points live on another device");
-    return curve_of(ctx->curve)->resident(out, ctx->d_points, npoints, scalars, scalars_mont != 0, ctx->wbits,
-                                          ctx->copies, ctx->npoints, 32, 255);
+    if (cur != ctx->device)
+        return rust_err(-(int)cudaErrorInvalidDevice, std::string(entry) + ": the points live on another device");
+    return curve_of(ctx->curve)->resident(out, ctx->d_points, npoints, scalars, mont, ctx->wbits, ctx->copies,
+                                          ctx->npoints, scalar_bytes, nbits);
 }
+
+extern "C" RustError sppark_b200_msm_ctx_invoke(sppark_b200_msm_ctx* ctx, void* out, const void* scalars,
+                                                size_t npoints, int scalars_mont)
+{   return ctx_invoke("msm_ctx_invoke", ctx, out, scalars, npoints, scalars_mont != 0, 32, 255);   }
 
 extern "C" RustError sppark_b200_msm_ctx_invoke_bits(sppark_b200_msm_ctx* ctx, void* out, const void* scalars,
                                                      size_t npoints, uint32_t scalar_bytes, uint32_t nbits)
 {
     if (ctx == nullptr) return rust_err(-(int)cudaErrorInvalidValue, "msm_ctx_invoke_bits: null context");
-    const curve_ops* c = curve_of(ctx->curve);
-    if (!scalar_format_ok(scalar_bytes, nbits))
-        return refuse(out, c->jacobian_bytes, "msm_ctx_invoke_bits: scalar_bytes must be 4, 8, 16 or 32 and "
-                                              "1 <= nbits <= min(255, 8 * scalar_bytes)");
-    if (npoints > ctx->npoints)
-        return rust_err(-(int)cudaErrorInvalidValue, "msm_ctx_invoke_bits: more scalars than preloaded points");
-    int cur = 0;
-    (void)cudaGetDevice(&cur);
-    if (cur != ctx->device) return rust_err(-(int)cudaErrorInvalidDevice, "msm_ctx_invoke_bits: the points live on another device");
-    return c->resident(out, ctx->d_points, npoints, scalars, false, ctx->wbits, ctx->copies, ctx->npoints,
-                       scalar_bytes, nbits);
+    const RustError e = check_scalar_format("msm_ctx_invoke_bits", curve_of(ctx->curve), out, scalar_bytes, nbits);
+    if (e.code != 0) return e;
+    return ctx_invoke("msm_ctx_invoke_bits", ctx, out, scalars, npoints, false, scalar_bytes, nbits);
 }
 
 extern "C" void sppark_b200_msm_ctx_free(sppark_b200_msm_ctx* ctx)

@@ -1,29 +1,7 @@
-// BLS12-381 G1 MSM: the drop-in entry points of poc/msm-cuda (see msm_host.cuh).
+// BLS12-381 G1 MSM (its drop-in entry points of poc/msm-cuda are in msm.cu) and the device self-test hooks.
 #include "msm_host.cuh"
 
-RustError msm_host_bls12_381(void* out, const void* points, size_t npoints, const void* scalars,
-                             size_t stride, bool has_flag, bool mont,
-                     uint32_t scalar_bytes, uint32_t nbits)
-{
-    return msm_host<ff::bls12_381_fp_t>(out, points, npoints, scalars, stride, has_flag,
-                                        mont ? scalars_from_mont<ff::bls12_381_fr_t> : nullptr, nullptr, nullptr,
-                     scalar_bytes, nbits);
-}
-RustError msm_dev_bls12_381(void* out, const void* d_points, size_t npoints, const void* d_scalars, void* stream,
-                  uint32_t scalar_bytes, uint32_t nbits)
-{   return msm_dev<ff::bls12_381_fp_t>(out, d_points, npoints, d_scalars, stream, scalar_bytes, nbits);   }
-
-RustError gen_points_bls12_381(void* d_out, size_t n, void* stream)
-{   return gen_points_dev<ff::bls12_381_g1_gen>(d_out, n, stream);   }
-RustError combine_bls12_381(void* out, const void* partials, size_t count)
-{   return combine_host<ff::bls12_381_fp_t>(out, partials, count);   }
-
-extern "C" RustError mult_pippenger(void* out, const void* points, size_t npoints, const void* scalars)
-{   return msm_host_bls12_381(out, points, npoints, scalars, 96, false, false, 32, 255);   }
-
-extern "C" RustError mult_pippenger_inf(void* out, const void* points, size_t npoints,
-                                        const void* scalars, size_t ffi_affine_sz)
-{   return msm_host_bls12_381(out, points, npoints, scalars, ffi_affine_sz, true, false, 32, 255);   }
+constexpr curve_ops curve_bls12_381 = curve_row<ff::bls12_381_g1_gen, ff::bls12_381_fr_t>();
 
 // ---- device self-test hook: element-wise field ops through the PTX arithmetic -------------
 // op 0 mul, 1 add, 2 sub, 3 sqr, 4 mul_shared, 5 sqr_shared, 6 msub_shared(x,y,y,x^2): host arrays
@@ -92,17 +70,6 @@ extern "C" RustError sppark_b200_selftest_field(int field, int op, size_t n, voi
     case 7: return selftest<ff::bls12_377_fr_t>(op, n, r, a, b);
     default: return rust_err(-(int)cudaErrorInvalidValue, "selftest: unknown field");
     }
-}
-
-RustError msm_preload_bls12_381(const void* points, size_t npoints, size_t stride, bool has_flag, void** d_points,
-                                uint32_t* copies, uint32_t* wbits)
-{   return msm_preload<ff::bls12_381_fp_t>(points, npoints, stride, has_flag, d_points, copies, wbits);   }
-RustError msm_resident_bls12_381(void* out, const void* d_points, size_t npoints, const void* scalars, bool mont,
-                                 uint32_t wbits, uint32_t copies, size_t stride,
-                       uint32_t scalar_bytes, uint32_t nbits)
-{
-    return msm_resident<ff::bls12_381_fp_t, ff::bls12_381_fr_t>(out, d_points, npoints, scalars, mont, wbits, copies, stride,
-                   scalar_bytes, nbits);
 }
 
 // ---- device self-test hook: the MSM's bucket sort alone (tests/test_msm_sort.py) -------------------
