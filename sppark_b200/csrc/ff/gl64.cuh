@@ -1,8 +1,10 @@
 // Goldilocks field  p = 2^64 - 2^32 + 1  (the reference's gl64_t, ff/gl64_t.cuh:39-298).
-// Memory format of the DATA is the reference's: one canonical uint64_t (< p), not Montgomery.
+// Memory format of the DATA is the reference's: one plain uint64_t, not Montgomery.  Contract of
+// the library's entry points on this field: an input word may be any uint64_t and stands for its value mod p
+// (callers such as Plonky2 keep non-canonical words); every output word is canonical (< p).
 //
 // Representation used by the NTT kernels:
-//  * data values travel as "loose" 64-bit residues (any uint64_t, value mod p);
+//  * data values travel as "loose" 64-bit residues (any uint64_t, value mod p), from load() on;
 //  * every CONSTANT the data is multiplied by (twiddles, coset powers, n^-1) is kept in
 //    Montgomery form c' = c * 2^64 mod p, canonical; mul(x, c') = x * c' * 2^-64 = x * c mod p,
 //    so products of data and constants are plain again and tables of constants are closed under

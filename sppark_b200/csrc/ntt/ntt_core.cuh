@@ -252,8 +252,11 @@ HD void phase_step(const K k, typename F::T* smem, uint32_t b, uint32_t tid)
                 if (m0 & (1u << t)) continue;
                 const uint32_t m1 = m0 | (1u << t);
                 T tt;
-                if (b + t == 0) {
-                    tt = x[m1];                                  // w = 1, value canonical since load
+                if (b == 0 && (m0 & ((1u << t) - 1)) == 0) {
+                    // w = 1 (j = 0 when b = 0): reduce instead of multiplying by one.  The operand
+                    // is loose -- a sum or difference, or at t = 0 a caller's word as loaded
+                    // (F::load) -- and add/sub need a canonical second operand
+                    tt = F::canon(x[m1]);
                 } else {
                     const uint32_t idx = ((m0 & ((1u << t) - 1)) << b) + j;
                     tt = F::mul(x[m1], tw[h + idx]);

@@ -1,7 +1,11 @@
 """Host-side mirror of the reference's ntt-cuda crate (poc/ntt-cuda/src/lib.rs:20-118):
 NTT / iNTT / coset_NTT / coset_iNTT, in place on a host array, through the C-ABI
 `compute_ntt`-style entry points.  Element type picks the field: uint64 = Goldilocks,
-uint32 = BabyBear (Montgomery words), as the reference's per-FEATURE builds do."""
+uint32 = BabyBear (Montgomery words), as the reference's per-FEATURE builds do.
+
+Input words: a Goldilocks word may be any uint64 and stands for its value mod p (non-canonical
+words, as Plonky2 keeps them, are accepted); BabyBear and the 256-bit fields take canonical
+Montgomery residues (< p), as the reference does.  Every entry here returns canonical words."""
 import numpy as np
 
 from . import _lib
