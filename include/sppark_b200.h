@@ -164,6 +164,27 @@ RustError sppark_b200_lde_batch_dev(int field, void *d_out, void *d_in, uint32_t
 RustError sppark_b200_ntt_batch(int field, size_t device_id, void *inout, uint32_t lg_domain_size,
                                 size_t batch, int ntt_order, int ntt_direction, int ntt_type);
 
+/* NTT and LDE down the COLUMNS of a row-major matrix (Goldilocks and BabyBear only; the 256-bit
+ * fields are refused with -cudaErrorInvalidValue): height = 2^lg_domain_size rows, `width` >= 1
+ * columns, element (i, c) at word i * width + c, in the field's memory format.  Column c of the result
+ * is exactly what the single-transform entry with the same order, direction and type returns for
+ * column c alone; no transpose is made.  lg == 0 or width == 0 is a no-op; a byte size that overflows
+ * size_t, an lg (or lg + lg_blowup) past the field's maximum, a bad order / direction / type, an
+ * unknown field or overlapping LDE buffers are rejected before any memory is touched.
+ *   ntt_matrix_dev: device memory, in place, enqueued on `stream`, not synchronised;
+ *   lde_matrix_dev: d_in = 2^lg x width evaluations, left holding each column's coefficients in
+ *                   bit-reversed row order (column c of d_in = row c of what lde_batch_dev leaves in
+ *                   its d_in); d_out = 2^(lg + lg_blowup) x width evaluations on the coset, natural
+ *                   order; no overlap with d_in; enqueued on `stream`;
+ *   ntt_matrix:     host memory, in place, synchronised: the whole matrix is uploaded, transformed and
+ *                   downloaded (pageable memory through the same staging as the other host entries). */
+RustError sppark_b200_ntt_matrix_dev(int field, void *d_inout, uint32_t lg_domain_size, size_t width,
+                                     int ntt_order, int ntt_direction, int ntt_type, void *stream);
+RustError sppark_b200_lde_matrix_dev(int field, void *d_out, void *d_in, uint32_t lg_domain_size,
+                                     uint32_t lg_blowup, size_t width, void *stream);
+RustError sppark_b200_ntt_matrix(int field, size_t device_id, void *inout, uint32_t lg_domain_size,
+                                 size_t width, int ntt_order, int ntt_direction, int ntt_type);
+
 /* ---- polynomial helpers (SURVEY.md section 8, row f4) ----------------------------------------------
  * The reference's polynomial/ templates and ff/batch_inversion.hpp for the NTT fields above.  All
  * arrays are DEVICE memory in the field's memory format (the format compute_ntt uses), the work is

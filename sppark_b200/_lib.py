@@ -61,6 +61,9 @@ _SIGS = {
     "sppark_b200_ntt_batch_dev": [C.c_int, C.c_void_p, C.c_uint32, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_void_p],
     "sppark_b200_lde_batch_dev": [C.c_int, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_size_t, C.c_void_p],
     "sppark_b200_ntt_batch": [C.c_int, C.c_size_t, C.c_void_p, C.c_uint32, C.c_size_t, C.c_int, C.c_int, C.c_int],
+    "sppark_b200_ntt_matrix_dev": [C.c_int, C.c_void_p, C.c_uint32, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_void_p],
+    "sppark_b200_lde_matrix_dev": [C.c_int, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_size_t, C.c_void_p],
+    "sppark_b200_ntt_matrix": [C.c_int, C.c_size_t, C.c_void_p, C.c_uint32, C.c_size_t, C.c_int, C.c_int, C.c_int],
     "sppark_b200_msm_sharded": [C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t],
     "sppark_b200_ntt_sharded": [C.c_int, C.c_void_p, C.c_uint32, C.c_int, C.c_void_p, C.c_size_t],
     "sppark_b200_selftest_word_field": [C.c_int, C.c_int, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p],

@@ -80,6 +80,34 @@ template<class F> bool launch_static(const Pass& d, const Tables<F>& tb, const t
         || try_shapes<F, 9, 5>(d, tb, in, out, ntiles, smem, stream);    // 2^27 = 9+9+9 (BabyBear's maximum)
 }
 
+// matrix passes: statically shaped kernels for the (lg_r, lg_w) tiles of the hot shapes (DESIGN.md
+// section 4.6), one per shape for all orders (KShape); any other shape runs the run-time shaped one
+template<class F, uint32_t R, uint32_t W>
+static bool try_matrix(const Pass& d, const Tables<F>& tb, const typename F::T* in, typename F::T* out,
+                       uint64_t width, uint32_t lg_n, cudaStream_t stream)
+{
+    if (d.lg_r != R || d.lg_w != W) return false;
+    launch_matrix_pass<F, KShape<R, W>>(d, tb, in, out, width, lg_n, stream);
+    return true;
+}
+
+template<class F> void launch_matrix(const Pass& d, const Tables<F>& tb, const typename F::T* in, typename F::T* out,
+                                     uint64_t width, uint32_t lg_n, cudaStream_t stream)
+{
+    if (try_matrix<F, 12, 2>(d, tb, in, out, width, lg_n, stream)          // 2^24, 2^23
+        || try_matrix<F, 11, 3>(d, tb, in, out, width, lg_n, stream)       // 2^22, 2^21
+        || try_matrix<F, 10, 4>(d, tb, in, out, width, lg_n, stream)       // 2^20, width > 8
+        || try_matrix<F, 10, 3>(d, tb, in, out, width, lg_n, stream)       // 2^20, width 5..8
+        || try_matrix<F, 8, 4>(d, tb, in, out, width, lg_n, stream))       // 2^16, width > 8 (2^12-element tiles)
+        return;
+    launch_matrix_pass<F, KDyn>(d, tb, in, out, width, lg_n, stream);
+}
+
+template void launch_matrix<gl64>(const Pass&, const Tables<gl64>&, const uint64_t*, uint64_t*, uint64_t, uint32_t, cudaStream_t);
+template void launch_matrix<bb31>(const Pass&, const Tables<bb31>&, const uint32_t*, uint32_t*, uint64_t, uint32_t, cudaStream_t);
+template struct NTTMatrix<gl64>;
+template struct NTTMatrix<bb31>;
+
 template bool launch_static<gl64>(const Pass&, const Tables<gl64>&, const uint64_t*, uint64_t*, uint32_t, size_t, cudaStream_t);
 template bool launch_static<bb31>(const Pass&, const Tables<bb31>&, const uint32_t*, uint32_t*, uint32_t, size_t, cudaStream_t);
 
@@ -513,5 +541,105 @@ extern "C" RustError sppark_b200_ntt_batch(int field, size_t device_id, void* in
     case SPPARK_FIELD_BN254_FR: return ntt_batch_host<ff::bn254_fr_ntt>(device_id, inout, lg, batch, order, direction, type);
     case SPPARK_FIELD_BLS12_377_FR: return ntt_batch_host<ff::bls12_377_fr_ntt>(device_id, inout, lg, batch, order, direction, type);
     default: return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_ntt_batch: unknown field");
+    }
+}
+
+// ---- NTT and LDE down the columns of a row-major matrix (ntt.cuh: NTTMatrix), Goldilocks and BabyBear ----
+static bool matrix_bad_args(int order, int direction, int type)
+{   return order < 0 || order > 4 || direction < 0 || direction > 1 || type < 0 || type > 1;   }
+
+template<class F>
+static RustError ntt_matrix_dev(void* d_inout, uint32_t lg, size_t width, int order, int direction, int type,
+                                void* stream)
+{
+    typedef ntt::NTT<F> N;
+    if (matrix_bad_args(order, direction, type))
+        return rust_err(-(int)cudaErrorInvalidValue, "ntt_matrix_dev: bad order/direction/type");
+    if (lg > (uint32_t)F::MAX_LG || !ntt::NTTMatrix<F>::fits(lg, width))
+        return rust_err(-(int)cudaErrorInvalidValue, "ntt_matrix_dev: lg_domain_size or width out of range for this field");
+    try {
+        ntt::NTTMatrix<F>::transform(gpu_of_current_device(), (typename F::T*)d_inout, lg, width,
+                                     (typename N::InputOutputOrder)order, (typename N::Direction)direction,
+                                     (typename N::Type)type, (cudaStream_t)stream);
+        return rust_ok();
+    } catch (const cuda_error& e) {
+        return rust_err(e.code(), e.what());
+    } catch (const std::exception& e) {
+        return rust_err(-1, e.what());
+    }
+}
+
+template<class F>
+static RustError lde_matrix_dev(void* d_out, void* d_in, uint32_t lg, uint32_t lg_blowup, size_t width, void* stream)
+{
+    try {
+        ntt::NTTMatrix<F>::LDE_dev(gpu_of_current_device(), (cudaStream_t)stream, (typename F::T*)d_out,
+                                   (typename F::T*)d_in, lg, lg_blowup, width);
+        return rust_ok();
+    } catch (const cuda_error& e) {
+        return rust_err(e.code(), e.what());
+    } catch (const std::exception& e) {
+        return rust_err(-1, e.what());
+    }
+}
+
+template<class F>
+static RustError ntt_matrix_host(size_t device_id, void* inout, uint32_t lg, size_t width, int order, int direction,
+                                 int type)
+{
+    typedef ntt::NTT<F> N;
+    if (matrix_bad_args(order, direction, type))
+        return rust_err(-(int)cudaErrorInvalidValue, "ntt_matrix: bad order/direction/type");
+    if (lg > (uint32_t)F::MAX_LG || !ntt::NTTMatrix<F>::fits(lg, width))
+        return rust_err(-(int)cudaErrorInvalidValue, "ntt_matrix: lg_domain_size or width out of range for this field");
+    if (lg == 0 || width == 0) return rust_ok();
+    try {
+        return ntt::NTTMatrix<F>::host(select_gpu((int)device_id), (typename F::T*)inout, lg, width,
+                                       (typename N::InputOutputOrder)order, (typename N::Direction)direction,
+                                       (typename N::Type)type);
+    } catch (const cuda_error& e) {
+        return rust_err(e.code(), e.what());
+    } catch (const std::exception& e) {
+        return rust_err(-1, e.what());
+    }
+}
+
+static RustError matrix_field_refused(int field, const char* entry)
+{
+    static const std::string wide = ": the matrix entries serve Goldilocks and BabyBear only, not the 256-bit fields";
+    static const std::string unknown = ": unknown field";
+    const bool is_wide = field == SPPARK_FIELD_BLS12_381_FR || field == SPPARK_FIELD_PALLAS_FR ||
+                         field == SPPARK_FIELD_VESTA_FR || field == SPPARK_FIELD_BN254_FR ||
+                         field == SPPARK_FIELD_BLS12_377_FR;
+    return rust_err(-(int)cudaErrorInvalidValue, (std::string(entry) + (is_wide ? wide : unknown)).c_str());
+}
+
+extern "C" RustError sppark_b200_ntt_matrix_dev(int field, void* d_inout, uint32_t lg, size_t width, int order,
+                                                int direction, int type, void* stream)
+{
+    switch (field) {
+    case SPPARK_FIELD_GL64: return ntt_matrix_dev<gl64>(d_inout, lg, width, order, direction, type, stream);
+    case SPPARK_FIELD_BB31: return ntt_matrix_dev<bb31>(d_inout, lg, width, order, direction, type, stream);
+    default: return matrix_field_refused(field, "sppark_b200_ntt_matrix_dev");
+    }
+}
+
+extern "C" RustError sppark_b200_lde_matrix_dev(int field, void* d_out, void* d_in, uint32_t lg, uint32_t lg_blowup,
+                                                size_t width, void* stream)
+{
+    switch (field) {
+    case SPPARK_FIELD_GL64: return lde_matrix_dev<gl64>(d_out, d_in, lg, lg_blowup, width, stream);
+    case SPPARK_FIELD_BB31: return lde_matrix_dev<bb31>(d_out, d_in, lg, lg_blowup, width, stream);
+    default: return matrix_field_refused(field, "sppark_b200_lde_matrix_dev");
+    }
+}
+
+extern "C" RustError sppark_b200_ntt_matrix(int field, size_t device_id, void* inout, uint32_t lg, size_t width,
+                                            int order, int direction, int type)
+{
+    switch (field) {
+    case SPPARK_FIELD_GL64: return ntt_matrix_host<gl64>(device_id, inout, lg, width, order, direction, type);
+    case SPPARK_FIELD_BB31: return ntt_matrix_host<bb31>(device_id, inout, lg, width, order, direction, type);
+    default: return matrix_field_refused(field, "sppark_b200_ntt_matrix");
     }
 }

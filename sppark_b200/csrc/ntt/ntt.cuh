@@ -69,9 +69,85 @@ pass_kernel_static(const Pass d, const Tables<F> tb, const typename F::T* in, ty
     }
 }
 
+// a pass over the columns of a row-major matrix (set_matrix, phase_load_matrix in ntt_core.cuh):
+// persistent CTAs walk the tiles i = t * ncb + cb (transform tile t, column block cb), so that
+// neighbouring CTAs read neighbouring column blocks of the same rows.  The sub-NTT twiddles are
+// staged once per CTA, by one bulk asynchronous copy (TMA) under the first tile load when the table
+// is whole 16-byte units, by the threads otherwise (sub-NTTs of 2 or 4 BabyBear words).  K is KDyn
+// (any shape) or KShape<R, W>.
+template<class F, class K>
+__global__ void __launch_bounds__(F::NTT_MAX_THREADS)
+matrix_pass_kernel(const Pass d, const Tables<F> tb, const typename F::T* in, typename F::T* out,
+                   uint64_t width, uint64_t ncb, uint64_t ntiles)
+{
+    typedef typename F::T T;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    T* smem = reinterpret_cast<T*>(smem_raw);
+    const uint32_t tid = threadIdx.x;
+    constexpr uint32_t LG_EPT = F::LG_EPT;
+    const K k{d};
+    const uint32_t R = k.lg_r();
+    const uint32_t nthreads = (R >= LG_EPT ? (1u << (R - LG_EPT)) : 1u) << k.lg_w();
+
+    __shared__ uint64_t tw_bar;
+    const uint32_t tw_bytes = (uint32_t)sizeof(T) << R;
+    const bool tma = tw_bytes % 16 == 0;
+    if (tma) {
+        if (tid == 0) mbar_init(&tw_bar, 1);
+        __syncthreads();
+        if (tid == 0) tma_load_1d(smem + (col_stride(R) << k.lg_w()), tb.dense, tw_bytes, &tw_bar);
+    } else {
+        phase_twiddles<F>(k, tb, smem, tid, nthreads);
+    }
+    bool tw_pending = tma;
+    for (uint64_t i = blockIdx.x; i < ntiles; i += gridDim.x) {
+        const uint64_t t = i / ncb, cb = i - t * ncb;
+        phase_load_matrix<F>(k, d, tb, in, smem, t, cb, width, tid, nthreads);
+        if (tw_pending) { mbar_wait(&tw_bar, 0); tw_pending = false; }
+        __syncthreads();
+#pragma unroll
+        for (uint32_t s = 0; s < step_count<F>(R); s++) {
+            if (s < R / LG_EPT) phase_step<F, K, LG_EPT>(k, smem, s * LG_EPT, tid);
+            else phase_step_dyn<F>(k, smem, s * LG_EPT, R - (R / LG_EPT) * LG_EPT, tid);
+            __syncthreads();
+        }
+        phase_store_matrix<F>(k, d, tb, out, smem, t, cb, width, tid, nthreads);
+        __syncthreads();
+    }
+}
+
+// one launch of matrix_pass_kernel<F, K>: as many CTAs as fit on the GPU at once, at most one per tile
+template<class F, class K>
+void launch_matrix_pass(const Pass& d, const Tables<F>& tb, const typename F::T* in, typename F::T* out,
+                        uint64_t width, uint32_t lg_n, cudaStream_t stream)
+{
+    int dev = 0;
+    CUDA_OK(cudaGetDevice(&dev));
+    static bool attr_done[64];
+    static int sms_of[64];
+    if (!attr_done[dev & 63]) {
+        // + the static mbarrier word <= 227 KiB
+        CUDA_OK(cudaFuncSetAttribute(matrix_pass_kernel<F, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
+        CUDA_OK(cudaDeviceGetAttribute(&sms_of[dev & 63], cudaDevAttrMultiProcessorCount, dev));
+        attr_done[dev & 63] = true;
+    }
+    const size_t smem = smem_elems(d) * sizeof(typename F::T);
+    const uint32_t threads = tile_threads<F>(d);
+    const uint64_t ncb = matrix_col_blocks(d, width), ntiles = ncb << (lg_n - d.lg_r);
+    uint32_t per_sm = smem <= 48 * 1024 ? 4 : smem <= 100 * 1024 ? 2 : 1;
+    while (per_sm > 1 && per_sm * threads > 2048) per_sm >>= 1;
+    const uint64_t cap = (uint64_t)sms_of[dev & 63] * per_sm;
+    matrix_pass_kernel<F, K><<<(uint32_t)(ntiles < cap ? ntiles : cap), threads, smem, stream>>>(
+        d, tb, in, out, width, ncb, ntiles);
+}
+
 // launcher table for the statically shaped passes; returns false if (d) has no static twin
 template<class F> bool launch_static(const Pass& d, const Tables<F>& tb, const typename F::T* in,
                                      typename F::T* out, uint32_t ntiles, size_t smem, cudaStream_t stream);
+// a matrix pass: the statically shaped kernel of d's (lg_r, lg_w) if there is one, else the
+// run-time shaped one (ntt.cu)
+template<class F> void launch_matrix(const Pass& d, const Tables<F>& tb, const typename F::T* in, typename F::T* out,
+                                     uint64_t width, uint32_t lg_n, cudaStream_t stream);
 // warp-autonomous pass (ntt_warp.cuh) for 4 <= d.lg_r <= 8, single-word fields; false otherwise
 template<class F> bool launch_warp(const gpu_t& gpu, const Pass& d, const Tables<F>& tb, const typename F::T* in,
                                    typename F::T* out, uint32_t ncols, cudaStream_t stream);
@@ -176,11 +252,35 @@ __global__ void lde_spread_kernel(typename F::T* out, const typename F::T* in, u
     }
 }
 
+// coset shift and LDE spread of a row-major matrix (coset_matrix_row, lde_spread_matrix_row): a block
+// of bx x by threads, bx (a power of two) along a row's columns, by rows at a time; one coset factor
+// per row and thread, no division per element
+template<class F>
+__global__ void coset_matrix_kernel(typename F::T* data, uint32_t lg_n, uint64_t width, bool bitrev,
+                                    const typename F::T* g0, const typename F::T* g1, const typename F::T* g2)
+{
+    const uint64_t rows = (uint64_t)1 << lg_n;
+    for (uint64_t r = (uint64_t)blockIdx.x * blockDim.y + threadIdx.y; r < rows; r += (uint64_t)gridDim.x * blockDim.y)
+        coset_matrix_row<F>(data, r, width, lg_n, bitrev, g0, g1, g2, threadIdx.x, blockDim.x);
+}
+
+template<class F>
+__global__ void lde_spread_matrix_kernel(typename F::T* out, const typename F::T* in, uint32_t lg_n, uint32_t lg_blowup,
+                                         uint64_t width, const typename F::T* g0, const typename F::T* g1,
+                                         const typename F::T* g2)
+{
+    const uint64_t rows = (uint64_t)1 << (lg_n + lg_blowup);
+    for (uint64_t r = (uint64_t)blockIdx.x * blockDim.y + threadIdx.y; r < rows; r += (uint64_t)gridDim.x * blockDim.y)
+        lde_spread_matrix_row<F>(out, in, r, width, lg_n, lg_blowup, g0, g1, g2, threadIdx.x, blockDim.x);
+}
+
 template<class F> struct FieldId;     // specialised in ntt.cu: cache key + shared-memory tile
+template<class F> struct NTTMatrix;
 
 template<class F>
 class NTT {
     typedef typename F::T T;
+    friend struct NTTMatrix<F>;       // shares the twiddle and coset tables
 public:
     enum class InputOutputOrder { NN, NR, RN, RR, BB };
     enum class Direction { forward, inverse };
@@ -626,6 +726,149 @@ public:
                 s.HtoD(d_inout, inout, n * sizeof(T));
             }
             NTT_internal(gpu, d_inout, lg_n, order, direction, type, s);
+            if (pageable) gpu.stager().DtoH(s, inout, d_inout, n * sizeof(T));
+            else s.DtoH(inout, d_inout, n * sizeof(T));
+            s.sync();
+        } catch (const cuda_error& e) {
+            try { gpu.sync(); } catch (...) {}
+            return rust_err(e.code(), e.what());
+        }
+        return rust_ok();
+    }
+};
+
+// NTT and LDE down the columns of a row-major 2^lg_n x width matrix, element (i, c) at word
+// i * width + c, single-word fields.  Column c of the result is what NTT::NTT_internal returns for
+// column c alone (same order, direction and type, the same coset exponents), without a transpose:
+// the passes of the single-transform plan read and write tiles of adjacent matrix columns
+// (set_matrix, matrix_pass_kernel).
+template<class F>
+struct NTTMatrix {
+    typedef typename F::T T;
+    typedef NTT<F> N;
+
+    // rejects a matrix whose byte size does not fit size_t (callers validate before any work)
+    static bool fits(uint32_t lg_n, size_t width)
+    {   return lg_n <= 30 && width <= (SIZE_MAX / sizeof(T)) >> lg_n;   }
+
+    // Tile shape, from the shape alone.  Every pass's sub-NTT is a digit of the single-transform plan
+    // (2^12 rows at most, two passes up to 2^24); next to it, as many adjacent matrix columns as fill
+    // a 2^14-element tile (the pass kernels' shared-memory tile), up to 64 and no more than the
+    // width.  At 2^24 that is 4 columns, 32-byte row chunks for Goldilocks and 16-byte ones for
+    // BabyBear; three passes of 2^8 rows with 16 columns were 15 % (Goldilocks) and 16 % (BabyBear)
+    // slower on H100 at 2^24 x 16: the third pass costs more than the narrow chunks.  Below 2^22
+    // elements in all the tile shrinks so that there are still >= 256 of them for the 132 SMs, as
+    // for the batched passes.  DESIGN.md section 4.6 has the measurements.
+    static uint32_t lg_tile(uint32_t lg_n, size_t width)
+    {
+        uint32_t lg_total = lg_n, lg_tile = FieldId<F>::lg_tile;
+        while (lg_total < 63 && (width >> (lg_total - lg_n)) > 1) lg_total++;   // floor(log2(width << lg_n))
+        if (lg_total < lg_tile + 8) lg_tile = lg_total > 18 ? lg_total - 8 : 10;
+        return lg_tile > FieldId<F>::lg_tile ? FieldId<F>::lg_tile : lg_tile;
+    }
+
+    static void coset_scale(const gpu_t& gpu, T* d, uint32_t lg_n, size_t width, bool bitrev, bool inverse,
+                            cudaStream_t stream)
+    {
+        const auto& ct = N::coset_tables(gpu, inverse, stream);
+        uint32_t bx = 1;
+        while (bx < 256 && bx < width) bx <<= 1;
+        const dim3 block(bx, 256 / bx);
+        const size_t blocks = (((size_t)1 << lg_n) + block.y - 1) / block.y, cap = (size_t)gpu.sm_count() * 8;
+        coset_matrix_kernel<F><<<(uint32_t)(blocks < cap ? blocks : cap), block, 0, stream>>>(d, lg_n, width, bitrev,
+                                                                                         ct.g0, ct.g1, ct.g2);
+        COUNT_LAUNCH();
+        CUDA_OK(cudaGetLastError());
+    }
+
+    // device-resident, in place, enqueued on `stream`, no synchronisation
+    static void transform(const gpu_t& gpu, T* d_inout, uint32_t lg_n, size_t width,
+                          typename N::InputOutputOrder order, typename N::Direction direction,
+                          typename N::Type type, cudaStream_t stream)
+    {
+        if (lg_n > (uint32_t)F::MAX_LG || !fits(lg_n, width))
+            throw cuda_error(-(int)cudaErrorInvalidValue, "NTT matrix: lg_domain_size or width out of range for this field");
+        if (lg_n == 0 || width == 0) return;
+        const bool inverse = direction == N::Direction::inverse;
+        const bool coset = type == N::Type::coset;
+        // coset exponents as NTT_internal: bit-reversed for RR although the data is in natural order
+        const bool in_rev = order != N::InputOutputOrder::NN && order != N::InputOutputOrder::NR;
+        const bool out_rev = order != N::InputOutputOrder::NN && order != N::InputOutputOrder::RN;
+        const uint32_t lg_t = lg_tile(lg_n, width);
+        Plan plan = make_plan(lg_n, (int)order, inverse, lg_t, /*max_lg_w=*/0, F::NTT_MAX_LG_R);
+        if (!set_matrix(plan, width, lg_t))
+            throw cuda_error(-(int)cudaErrorInvalidValue, "NTT matrix: this plan has no matrix form");
+
+        if (coset && !inverse) coset_scale(gpu, d_inout, lg_n, width, in_rev, false, stream);
+        const Tables<F>& tb = N::tables(gpu, lg_n, inverse, stream);
+        T* scratch = nullptr;
+        if (plan.needs_scratch)
+            CUDA_OK(cudaMallocAsync((void**)&scratch, (sizeof(T) * width) << lg_n, stream));
+        T* buf[2] = {d_inout, scratch};
+        g_profile.reset();
+        for (const Pass& d : plan.passes) {
+            g_profile.mark("pass", stream);
+            launch_matrix<F>(d, tb, buf[d.src], buf[d.dst], width, lg_n, stream);
+            COUNT_LAUNCH();
+            CUDA_OK(cudaGetLastError());
+        }
+        g_profile.mark("end", stream);
+        if (scratch) CUDA_OK(cudaFreeAsync(scratch, stream));
+        if (coset && inverse) coset_scale(gpu, d_inout, lg_n, width, out_rev, true, stream);
+    }
+
+    // LDE of every column, enqueued on `stream`: d_in (2^lg_n x width evaluations) is left holding each
+    // column's coefficients in bit-reversed row order; d_out receives 2^(lg_n + lg_blowup) x width
+    // evaluations on the coset, natural order.  The same composition as NTT::LDE_batch_dev: inverse NR,
+    // the spread with the coset shift, forward RN
+    static void LDE_dev(const gpu_t& gpu, cudaStream_t stream, T* d_out, T* d_in, uint32_t lg_n, uint32_t lg_blowup,
+                        size_t width)
+    {
+        if (lg_n > 30 || lg_blowup > 30)
+            throw cuda_error(-(int)cudaErrorInvalidValue, "LDE matrix: lg_domain_size + lg_blowup out of range for this field");
+        const uint32_t lg_ext = lg_n + lg_blowup;
+        if (lg_ext > (uint32_t)F::MAX_LG || !fits(lg_ext, width))
+            throw cuda_error(-(int)cudaErrorInvalidValue, "LDE matrix: lg_domain_size + lg_blowup out of range for this field");
+        if (lg_n == 0 || width == 0) return;
+        // the spread reads all of d_in while writing d_out: the two must not overlap
+        const size_t n_in = width << lg_n, n_out = width << lg_ext;
+        if (d_in < d_out + n_out && d_out < d_in + n_in)
+            throw cuda_error(-(int)cudaErrorInvalidValue, "LDE matrix: d_out overlaps d_in");
+        transform(gpu, d_in, lg_n, width, N::InputOutputOrder::NR, N::Direction::inverse, N::Type::standard, stream);
+        const auto& ct = N::coset_tables(gpu, false, stream);
+        uint32_t bx = 1;
+        while (bx < 256 && bx < width) bx <<= 1;
+        const dim3 block(bx, 256 / bx);
+        const size_t blocks = (((size_t)1 << lg_ext) + block.y - 1) / block.y, cap = (size_t)gpu.sm_count() * 8;
+        lde_spread_matrix_kernel<F><<<(uint32_t)(blocks < cap ? blocks : cap), block, 0, stream>>>(
+            d_out, d_in, lg_n, lg_blowup, width, ct.g0, ct.g1, ct.g2);
+        COUNT_LAUNCH();
+        CUDA_OK(cudaGetLastError());
+        transform(gpu, d_out, lg_ext, width, N::InputOutputOrder::RN, N::Direction::forward, N::Type::standard, stream);
+    }
+
+    // host memory, in place, synchronised: the whole matrix is uploaded, transformed and downloaded
+    // (pageable memory through the pinned staging ring, as in NTT::Base)
+    static RustError host(const gpu_t& gpu, T* inout, uint32_t lg_n, size_t width, typename N::InputOutputOrder order,
+                          typename N::Direction direction, typename N::Type type)
+    {
+        if (lg_n > (uint32_t)F::MAX_LG || !fits(lg_n, width))       // before touching the caller's buffer
+            return rust_err(-(int)cudaErrorInvalidValue, "NTT matrix: lg_domain_size or width out of range for this field");
+        if (lg_n == 0 || width == 0) return rust_ok();
+        try {
+            gpu.select();
+            const stream_t& s = gpu[0];
+            const size_t n = width << lg_n;
+            dev_ptr_t<T> d_inout(n, s);
+            const bool pageable = n * sizeof(T) >= ((size_t)8 << 20) && stager_t::is_pageable(inout);
+            std::unique_lock<std::mutex> stage_lock(gpu.stage_mtx, std::defer_lock);
+            if (pageable) {
+                stage_lock.lock();
+                gpu.stager().HtoD(s, d_inout, inout, n * sizeof(T));
+            } else {
+                s.HtoD(d_inout, inout, n * sizeof(T));
+            }
+            transform(gpu, d_inout, lg_n, width, order, direction, type, s);
             if (pageable) gpu.stager().DtoH(s, inout, d_inout, n * sizeof(T));
             else s.DtoH(inout, d_inout, n * sizeof(T));
             s.sync();

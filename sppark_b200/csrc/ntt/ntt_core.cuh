@@ -109,6 +109,18 @@ struct KStat {
     static HD constexpr bool out_rev() { return OREV; }
     static HD constexpr uint32_t tw_mode() { return TW; }
 };
+// tile shape fixed at compile time, order and twiddle flags read from the descriptor (the matrix
+// passes: one instantiation per shape serves every order)
+template<uint32_t R, uint32_t W>
+struct KShape {
+    const Pass& d;
+    HD explicit KShape(const Pass& d_) : d(d_) {}
+    static HD constexpr uint32_t lg_r() { return R; }
+    static HD constexpr uint32_t lg_w() { return W; }
+    HD bool in_rev() const { return d.in_rev != 0; }
+    HD bool out_rev() const { return d.out_rev != 0; }
+    HD uint32_t tw_mode() const { return d.tw_mode; }
+};
 
 // Shared-memory placement of row `i` of column `c`: an XOR swizzle of the low four index bits
 // with bits 4-7, bits 8-11 and the column, so that a half-warp (sixteen 8-byte words = all 32
@@ -333,6 +345,114 @@ HD void phase_store(const K k, const Pass& d, const Tables<F>& tb, typename F::T
             out[obase + row_off + ((uint64_t)c << d.out_lg_sc)] = F::canon(x);
         }
     }
+}
+
+// ---- matrix layout: the transforms are the columns of a row-major 2^n x width matrix ---------
+// A matrix pass runs the plan of a single transform (make_plan with one transform column per
+// tile, set_matrix in ntt_plan.hpp) and reads its tile columns from 2^lg_w ADJACENT matrix columns
+// at one transform position: tile (t, cb) holds rows tile_base(t) + (row << lg_sa) of matrix
+// columns cb * 2^lg_w + c, element (pos, col) at word pos * width + col.  Every tile row is then a
+// contiguous run of 2^lg_w words, at any pass stride.  The inter-pass twiddle depends on the
+// transform position only: its column is the tile's (one per tile) and the factor the row's, shared
+// by all matrix columns.  Columns past `width` are masked.  The butterflies (phase_step) are the
+// same; consecutive threads walk matrix columns, the strided mapping of phase_load / phase_store.
+template<class F, class K>
+HD void phase_load_matrix(const K k, const Pass& d, const Tables<F>& tb, const typename F::T* in,
+                          typename F::T* smem, uint64_t t, uint64_t cb, uint64_t width,
+                          uint32_t tid, uint32_t nthreads)
+{
+    typedef typename F::T T;
+    const uint32_t R = k.lg_r(), LW = k.lg_w(), n_el = (1u << R) << LW, cs = col_stride(R);
+    const uint64_t base = tile_base((uint32_t)t, d.in_lg_tlo, d.in_tl, d.in_th), col0 = cb << LW;
+    const uint32_t colv = k.tw_mode() == TW_LOAD ? tw_column_value(d, base) : 0;
+    constexpr uint32_t EPT = 1u << F::LG_EPT;
+    T v[EPT];
+#pragma unroll
+    for (uint32_t l = 0; l < EPT; l++) {
+        uint32_t e = l * nthreads + tid;
+        v[l] = T{};
+        if (e < n_el) {
+            uint32_t a = e >> LW, c = e & ((1u << LW) - 1);
+            if (col0 + c < width)
+                v[l] = in[(base + ((uint64_t)a << d.in_lg_sa)) * width + col0 + c];
+        }
+    }
+#pragma unroll
+    for (uint32_t l = 0; l < EPT; l++) {
+        uint32_t e = l * nthreads + tid;
+        if (e < n_el) {
+            uint32_t a = e >> LW, c = e & ((1u << LW) - 1);
+            T x = F::load(v[l]);
+            uint32_t nat = k.in_rev() ? brev32(a, R) : a;          // natural row index
+            if (k.tw_mode() == TW_LOAD)
+                x = F::mul(x, twiddle<F>(tb, (nat * colv) << d.tw_lsh));
+            smem[c * cs + swz(brev32(nat, R), c, R)] = x;            // DIT wants bit-reversed rows
+        }
+    }
+}
+
+template<class F, class K>
+HD void phase_store_matrix(const K k, const Pass& d, const Tables<F>& tb, typename F::T* out,
+                           const typename F::T* smem, uint64_t t, uint64_t cb, uint64_t width,
+                           uint32_t tid, uint32_t nthreads)
+{
+    typedef typename F::T T;
+    const uint32_t R = k.lg_r(), LW = k.lg_w(), n_el = (1u << R) << LW, cs = col_stride(R);
+    const uint64_t ibase = tile_base((uint32_t)t, d.in_lg_tlo, d.in_tl, d.in_th);
+    const uint64_t obase = tile_base((uint32_t)t, d.out_lg_tlo, d.out_tl, d.out_th), col0 = cb << LW;
+    const uint32_t colv = k.tw_mode() == TW_STORE ? tw_column_value(d, ibase) : 0;
+    constexpr uint32_t EPT = 1u << F::LG_EPT;
+#pragma unroll
+    for (uint32_t l = 0; l < EPT; l++) {
+        uint32_t e = l * nthreads + tid;
+        if (e < n_el) {
+            uint32_t v = e >> LW, c = e & ((1u << LW) - 1);
+            uint32_t ka = k.out_rev() ? brev32(v, R) : v;          // natural output row
+            T x = smem[c * cs + swz(ka, c, R)];
+            if (k.tw_mode() == TW_STORE)
+                x = F::mul(x, twiddle<F>(tb, (ka * colv) << d.tw_lsh));
+            if (d.scale)
+                x = F::mul(x, tb.ninv);
+            if (col0 + c < width)
+                out[(obase + ((uint64_t)v << d.out_lg_sa)) * width + col0 + c] = F::canon(x);
+        }
+    }
+}
+
+// Coset shift and LDE spread of a matrix, one row at a time (each row is one transform position,
+// so one factor serves the whole row); columns c0, c0 + cstep, ... of the row.
+//   coset:  row i *= g^e(i), e(i) = i, or brev(i) over lg_n bits
+//   spread: output row r of 2^(lg_n + lg_blowup) = input row r >> lg_blowup times g^brev(r >> lg_blowup)
+//           when the low lg_blowup bits of r are zero, zero otherwise
+template<class F>
+HD void coset_matrix_row(typename F::T* data, uint64_t i, uint64_t width, uint32_t lg_n, bool bitrev,
+                         const typename F::T* g0, const typename F::T* g1, const typename F::T* g2,
+                         uint64_t c0, uint64_t cstep)
+{
+    typedef typename F::T T;
+    const T f = coset_mul<F>(F::one(), i, lg_n, bitrev, g0, g1, g2);
+    T* row = data + i * width;
+    for (uint64_t c = c0; c < width; c += cstep)
+        row[c] = F::canon(F::mul(F::load(row[c]), f));
+}
+
+template<class F>
+HD void lde_spread_matrix_row(typename F::T* out, const typename F::T* in, uint64_t r, uint64_t width,
+                              uint32_t lg_n, uint32_t lg_blowup,
+                              const typename F::T* g0, const typename F::T* g1, const typename F::T* g2,
+                              uint64_t c0, uint64_t cstep)
+{
+    typedef typename F::T T;
+    T* orow = out + r * width;
+    if (r & ((1u << lg_blowup) - 1)) {
+        for (uint64_t c = c0; c < width; c += cstep) orow[c] = T{};
+        return;
+    }
+    const uint64_t i = r >> lg_blowup;
+    const T f = coset_mul<F>(F::one(), i, lg_n, true, g0, g1, g2);
+    const T* irow = in + i * width;
+    for (uint64_t c = c0; c < width; c += cstep)
+        orow[c] = F::canon(F::mul(F::load(irow[c]), f));
 }
 
 }  // namespace ntt

@@ -170,6 +170,32 @@ inline bool set_batch(Plan& plan, uint64_t batch)
     return true;
 }
 
+// ---- the columns of a row-major 2^lg_n x width matrix (phase_load_matrix / phase_store_matrix) --
+// Turns a plan of make_plan(lg_n, order, inverse, ., /*max_lg_w=*/0, max_lg_r) -- one transform
+// column per tile, which is a complete plan of one transform -- into the same transform down every
+// column of the matrix.  The transform addressing terms stay as they are; d.lg_w now counts the
+// ADJACENT MATRIX COLUMNS a tile holds: as many as fill 2^lg_tile elements next to the pass's 2^lg_r
+// rows, at most 2^MATRIX_MAX_LG_W, and no more than `width` needs.  A pass has 2^(lg_n - lg_r) x
+// matrix_col_blocks() tiles.  Returns false for a plan with several transform columns per tile or
+// with slab / peer routing.
+constexpr uint32_t MATRIX_MAX_LG_W = 6;
+
+inline bool set_matrix(Plan& plan, uint64_t width, uint32_t lg_tile)
+{
+    for (const Pass& d : plan.passes)
+        if (d.lg_w || d.out_split_bits || d.peer_on || d.tw_col_offset) return false;
+    uint32_t lg_width = 0;                                // ceil(log2(width)), capped
+    while (lg_width < MATRIX_MAX_LG_W && (1ull << lg_width) < width) lg_width++;
+    for (Pass& d : plan.passes) {
+        const uint32_t lw = lg_tile > d.lg_r ? lg_tile - d.lg_r : 0;
+        d.lg_w = lw < lg_width ? lw : lg_width;
+    }
+    return true;
+}
+
+inline uint64_t matrix_col_blocks(const Pass& d, uint64_t width)
+{   return (width + (1ull << d.lg_w) - 1) >> d.lg_w;   }
+
 // ---- slab-sharded transform over G = 2^lg_g ranks, ONE all-to-all ---------------------------
 // N = N1 x N2 (N1 = 2^s1 rows, N2 = 2^s2 columns, x[j1*N2 + j2]).  Rank r owns the columns
 // j2 in [r*N2/G, (r+1)*N2/G) of the input, stored locally as a row-major [N1][N2/G] matrix, and

@@ -161,3 +161,65 @@ def lde_batch_dev(d_in, lg_blowup, field=None, stream=None):
         err = _lib.lib().sppark_b200_lde_batch_dev(field, out.data_ptr(), d_in.data_ptr(), lg, lg_blowup, batch, s)
     _lib.check(err)
     return out
+
+
+def _matrix_shape(shape, itemsize, field):
+    """(lg, width) of a (2^lg, width) matrix of Goldilocks (8-byte) or BabyBear (4-byte) words; the
+    element size must be the field's word size, or the library would run past the buffer"""
+    if field not in (GL64, BB31):
+        raise ValueError(f"field {field}: the matrix entries serve Goldilocks and BabyBear only")
+    if itemsize != (4 if field == BB31 else 8):
+        raise ValueError(f"{itemsize}-byte elements do not match field {field}")
+    if len(shape) != 2:
+        raise ValueError("matrices are (2^lg, width) arrays")
+    n, width = int(shape[0]), int(shape[1])
+    if n == 0 or n & (n - 1):
+        raise ValueError("matrix height is not a power of 2")
+    return n.bit_length() - 1, width
+
+
+def ntt_matrix(device_id, inout, order=NN, direction=FORWARD, typ=STANDARD, field=None):
+    """The transform down every column of a writable C-contiguous (2^lg, width) array (uint64 =
+    Goldilocks, uint32 = BabyBear), in place: column c comes out as NTT/iNTT/coset_* would return it
+    alone.  No transpose is made.  Synchronised."""
+    if not isinstance(inout, np.ndarray) or not inout.flags["C_CONTIGUOUS"] or not inout.flags["WRITEABLE"]:
+        raise ValueError("inout must be a writable C-contiguous numpy array")
+    if field is None:
+        if inout.dtype not in (np.uint64, np.uint32):
+            raise ValueError("inout must be uint64 (Goldilocks) or uint32 (BabyBear)")
+        field = _field_of(inout)
+    lg, width = _matrix_shape(inout.shape, inout.itemsize, field)
+    _lib.check(_lib.lib().sppark_b200_ntt_matrix(field, device_id, inout.ctypes.data, lg, width,
+                                                 order, direction, typ))
+
+
+def ntt_matrix_dev(tensor, order=NN, direction=FORWARD, typ=STANDARD, field=None, stream=None):
+    """ntt_matrix on a contiguous (2^lg, width) CUDA torch tensor: in place, enqueued on torch's
+    current stream (or `stream`), not synchronised."""
+    import torch
+    if not tensor.is_cuda or not tensor.is_contiguous():
+        raise ValueError("tensor must be a contiguous CUDA tensor")
+    field = _dev_field(tensor, field)
+    lg, width = _matrix_shape(tuple(tensor.shape), tensor.element_size(), field)
+    with torch.cuda.device(tensor.device):
+        s = stream if stream is not None else torch.cuda.current_stream().cuda_stream
+        err = _lib.lib().sppark_b200_ntt_matrix_dev(field, tensor.data_ptr(), lg, width, order, direction, typ, s)
+    _lib.check(err)
+
+
+def lde_matrix_dev(d_in, lg_blowup, field=None, stream=None):
+    """LDE of every column of a contiguous (2^lg, width) CUDA tensor: returns a new
+    (2^(lg + lg_blowup), width) tensor whose column c is what LDE returns for column c, and leaves
+    each column's coefficients, in bit-reversed row order, in d_in.  Enqueued on torch's current
+    stream (or `stream`), not synchronised."""
+    import torch
+    if not d_in.is_cuda or not d_in.is_contiguous():
+        raise ValueError("d_in must be a contiguous CUDA tensor")
+    field = _dev_field(d_in, field)
+    lg, width = _matrix_shape(tuple(d_in.shape), d_in.element_size(), field)
+    out = torch.empty(((1 << lg) << lg_blowup, width), dtype=d_in.dtype, device=d_in.device)
+    with torch.cuda.device(d_in.device):
+        s = stream if stream is not None else torch.cuda.current_stream().cuda_stream
+        err = _lib.lib().sppark_b200_lde_matrix_dev(field, out.data_ptr(), d_in.data_ptr(), lg, lg_blowup, width, s)
+    _lib.check(err)
+    return out
