@@ -295,6 +295,25 @@ RustError sppark_b200_msm_dev(int curve, void *out_jacobian, const void *d_point
  * to min(scalar_bytes, 16) bytes, each scalar is read with one load of its width. */
 RustError sppark_b200_msm_dev_bits(int curve, void *out_jacobian, const void *d_points, size_t npoints,
                                    const void *d_scalars, uint32_t scalar_bytes, uint32_t nbits, void *stream);
+/* Batched MSM: B = batch scalar vectors of npoints scalars each, against one point set, in one call.
+ * Vector b is the scalars [b * npoints, (b + 1) * npoints) in the small-scalar format of
+ * sppark_b200_msm_bits (scalar_bytes = 4, 8, 16 or 32, plain integers -- not Montgomery form --,
+ * bits from nbits up ignored; 32 and 255 for full-width scalars).  out_jacobians: HOST array of batch
+ * Jacobian points (batch * jacobian_bytes); result b is the same group element as the single entry
+ * with vector b.  The vectors run in groups that share one sort, accumulate, reduce and finish.
+ * batch == 0 is a no-op; npoints == 0 gives batch points at infinity.  A bad format, npoints past the
+ * context's count, batch * npoints * scalar_bytes overflowing size_t or misaligned device scalars are
+ * refused with -cudaErrorInvalidValue before any device work, every output set to infinity (not with
+ * a null context or an unknown curve: the output size is then unknown, and nothing is written).
+ *   _ctx_invoke_batch: host scalars against the first npoints preloaded points of a plain or
+ *     precomputed context; the scalars of the next group are uploaded while a group computes.
+ *   _dev_batch: device points and scalars (aligned as for sppark_b200_msm_dev_bits); the work runs on
+ *     `stream`, which is synchronised before return. */
+RustError sppark_b200_msm_ctx_invoke_batch(sppark_b200_msm_ctx *ctx, void *out_jacobians, const void *scalars,
+                                           size_t npoints, size_t batch, uint32_t scalar_bytes, uint32_t nbits);
+RustError sppark_b200_msm_dev_batch(int curve, void *out_jacobians, const void *d_points, size_t npoints,
+                                    const void *d_scalars, size_t batch, uint32_t scalar_bytes, uint32_t nbits,
+                                    void *stream);
 
 /* synthetic inputs: d_out[i] = (i+1)*G as packed affine points in DEVICE memory (the role of
  * util::generate_points_scalars, poc/msm-cuda/src/util.rs:11-38); enqueued on `stream`. */

@@ -53,6 +53,10 @@ _SIGS = {
     "sppark_b200_msm_dev_bits": [C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint32, C.c_uint32,
                                  C.c_void_p],
     "sppark_b200_msm_ctx_invoke_bits": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint32],
+    "sppark_b200_msm_ctx_invoke_batch": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_uint32,
+                                         C.c_uint32],
+    "sppark_b200_msm_dev_batch": [C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_uint32,
+                                  C.c_uint32, C.c_void_p],
     "sppark_b200_generate_points_dev": [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p],
     "sppark_b200_msm_combine": [C.c_int, C.c_void_p, C.c_void_p, C.c_size_t],
     "sppark_b200_selftest_field": [C.c_int, C.c_int, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p],

@@ -18,6 +18,12 @@ struct curve_ops {
                          uint32_t* copies, uint32_t* wbits);
     RustError (*resident)(void* out, const void* d_points, size_t npoints, const void* scalars, bool mont,
                           uint32_t wbits, uint32_t copies, size_t copy_stride, uint32_t scalar_bytes, uint32_t nbits);
+    // batches: `batch` vectors of npoints scalars one after the other, one Jacobian point per vector
+    RustError (*resident_batch)(void* out, const void* d_points, size_t npoints, const void* scalars, size_t batch,
+                                bool mont, uint32_t wbits, uint32_t copies, size_t copy_stride, uint32_t scalar_bytes,
+                                uint32_t nbits);
+    RustError (*dev_batch)(void* out, const void* d_points, size_t npoints, const void* d_scalars, size_t batch,
+                           void* stream, uint32_t scalar_bytes, uint32_t nbits);
     size_t affine_bytes, jacobian_bytes;        // packed {X, Y} and {X, Y, Z}
 };
 

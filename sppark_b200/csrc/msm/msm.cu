@@ -251,6 +251,70 @@ extern "C" RustError sppark_b200_msm_ctx_invoke_bits(sppark_b200_msm_ctx* ctx, v
     return ctx_invoke("msm_ctx_invoke_bits", ctx, out, scalars, npoints, false, scalar_bytes, nbits);
 }
 
+// ---- batches: many scalar vectors against one point set -----------------------------------------
+// A refusal sets all `batch` outputs to infinity, where their size is known and fits a size_t.
+static RustError refuse_batch(void* out, size_t batch, size_t jacobian_bytes, const std::string& msg)
+{
+    if (out && batch <= SIZE_MAX / jacobian_bytes) memset(out, 0, batch * jacobian_bytes);
+    return rust_err(-(int)cudaErrorInvalidValue, msg);
+}
+
+// the checks of both batch entries, before any device work; code 0 and *done = false when the call goes on
+static RustError check_batch(const char* entry, const curve_ops* c, void* out, size_t npoints, size_t batch,
+                             uint32_t scalar_bytes, uint32_t nbits, bool* done)
+{
+    *done = true;
+    const std::string e(entry);
+    const RustError f = check_scalar_format(entry, c, nullptr, scalar_bytes, nbits);
+    if (f.code != 0) {
+        if (out && batch <= SIZE_MAX / c->jacobian_bytes) memset(out, 0, batch * c->jacobian_bytes);
+        return f;
+    }
+    if (batch > SIZE_MAX / c->jacobian_bytes || (npoints && batch > SIZE_MAX / npoints / scalar_bytes))
+        return refuse_batch(out, batch, c->jacobian_bytes, e + ": batch * npoints * scalar_bytes overflows");
+    if (batch == 0) return rust_ok();
+    if (out == nullptr) return rust_err(-(int)cudaErrorInvalidValue, e + ": null output");
+    *done = false;
+    return rust_ok();
+}
+
+extern "C" RustError sppark_b200_msm_ctx_invoke_batch(sppark_b200_msm_ctx* ctx, void* out_jacobians,
+                                                      const void* scalars, size_t npoints, size_t batch,
+                                                      uint32_t scalar_bytes, uint32_t nbits)
+{
+    if (ctx == nullptr) return rust_err(-(int)cudaErrorInvalidValue, "msm_ctx_invoke_batch: null context");
+    const curve_ops* c = curve_of(ctx->curve);
+    bool done;
+    const RustError e = check_batch("msm_ctx_invoke_batch", c, out_jacobians, npoints, batch, scalar_bytes, nbits, &done);
+    if (e.code != 0 || done) return e;
+    if (npoints > ctx->npoints)
+        return refuse_batch(out_jacobians, batch, c->jacobian_bytes, "msm_ctx_invoke_batch: more scalars than preloaded points");
+    int cur = 0;
+    (void)cudaGetDevice(&cur);
+    if (cur != ctx->device) {
+        memset(out_jacobians, 0, batch * c->jacobian_bytes);
+        return rust_err(-(int)cudaErrorInvalidDevice, "msm_ctx_invoke_batch: the points live on another device");
+    }
+    return c->resident_batch(out_jacobians, ctx->d_points, npoints, scalars, batch, false, ctx->wbits, ctx->copies,
+                             ctx->npoints, scalar_bytes, nbits);
+}
+
+extern "C" RustError sppark_b200_msm_dev_batch(int curve, void* out_jacobians, const void* d_points, size_t npoints,
+                                               const void* d_scalars, size_t batch, uint32_t scalar_bytes,
+                                               uint32_t nbits, void* stream)
+{
+    const curve_ops* c = curve_of(curve);
+    if (c == nullptr) return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_msm_dev_batch: unknown curve");
+    bool done;
+    const RustError e = check_batch("sppark_b200_msm_dev_batch", c, out_jacobians, npoints, batch, scalar_bytes, nbits,
+                                    &done);
+    if (e.code != 0 || done) return e;
+    if ((uintptr_t)d_scalars % (scalar_bytes < 16 ? scalar_bytes : 16) != 0)   // one aligned load per scalar
+        return refuse_batch(out_jacobians, batch, c->jacobian_bytes, "sppark_b200_msm_dev_batch: d_scalars must be "
+                                                                     "aligned to min(scalar_bytes, 16) bytes");
+    return c->dev_batch(out_jacobians, d_points, npoints, d_scalars, batch, stream, scalar_bytes, nbits);
+}
+
 extern "C" void sppark_b200_msm_ctx_free(sppark_b200_msm_ctx* ctx)
 {
     if (ctx == nullptr) return;

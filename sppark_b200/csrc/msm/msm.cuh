@@ -73,6 +73,7 @@ __device__ uint32_t block_exclusive_scan(uint32_t len, Load load, Visit visit)
 // pass 1: bin histogram of the windows [w0, w0 + wpg) of group blockIdx.y in shared memory, one
 // global atomic per non-zero counter per CTA; a warp adds equal bins once (all scalars equal:
 // every lane of the warp hits one counter).  With a table every digit is walked: its set is w mod V.
+// A batch walks the vectors whose sets meet [w0, w1).
 // One instantiation per scalar width SW (cfg.swords words), each scalar read with one load of its width.
 template<uint32_t SW>
 __global__ void __launch_bounds__(HIST_THREADS)
@@ -80,19 +81,23 @@ bin_hist_kernel(const Config cfg, uint32_t lg_bins, const uint32_t* scalars, uin
 {
     extern __shared__ uint32_t hist[];
     const uint32_t w0 = blockIdx.y * wpg, w1 = min(w0 + wpg, cfg.nwins), nctr = (w1 - w0) << lg_bins;
-    const uint32_t d_end = cfg.copies > 1 ? digit_count(cfg) : w1;
+    const uint32_t V = vec_sets(cfg), D = digit_count(cfg);
     const uint32_t lane = threadIdx.x & 31;
     for (uint32_t k = threadIdx.x; k < nctr; k += blockDim.x) hist[k] = 0;
     __syncthreads();
-    for (uint32_t i0 = blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < cfg.npoints; i0 += gridDim.x * blockDim.x) {
-        const uint32_t i = i0 + lane;                               // whole warps iterate together
-        for_each_digit<SW>(cfg, lg_bins, scalars, i, i < cfg.npoints, d_end,
-                       [&](uint32_t w, bool nz, uint32_t bin, uint32_t, uint32_t) {
-            if (w < w0 || w >= w1) return;                          // the same for the whole warp
-            const uint32_t key = nz ? bin - (w0 << lg_bins) : ~0u;
-            const uint32_t peers = __match_any_sync(0xffffffffu, key);
-            if (nz && lane == __ffs(peers) - 1) atomicAdd(&hist[key], __popc(peers));
-        });
+    for (uint32_t g = w0 / V; g * V < w1; g++) {
+        // without a table digit w of vector g lands in set gV + w: the digits of sets past w1 are not walked
+        const uint32_t d_end = cfg.copies > 1 ? D : min(D, w1 - g * V);
+        for (uint32_t i0 = blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < cfg.npoints; i0 += gridDim.x * blockDim.x) {
+            const uint32_t i = i0 + lane;                           // whole warps iterate together
+            for_each_digit<SW>(cfg, lg_bins, scalars, i, i < cfg.npoints, d_end,
+                           [&](uint32_t w, bool nz, uint32_t bin, uint32_t, uint32_t) {
+                if (w < w0 || w >= w1) return;                      // the same for the whole warp
+                const uint32_t key = nz ? bin - (w0 << lg_bins) : ~0u;
+                const uint32_t peers = __match_any_sync(0xffffffffu, key);
+                if (nz && lane == __ffs(peers) - 1) atomicAdd(&hist[key], __popc(peers));
+            }, g);
+        }
     }
     __syncthreads();
     for (uint32_t k = threadIdx.x; k < nctr; k += blockDim.x)
@@ -110,24 +115,26 @@ bin_scan_kernel(uint32_t lg_bins, const uint32_t* bin_count, uint32_t* bin_base,
 
 // pass 2: every (point, window) entry appended at its bin's cursor, one reservation per distinct
 // bin per warp.  All windows in one pass: the open frontier is one partly written line per bin
-// (W * 2^lg_bins * 128 B, 13.6 MB at 2^26 points), so lines fill in L2 and leave whole.
+// (nwins * 2^lg_bins * 128 B, 13.6 MB at 2^26 points; a batch's group is sized to keep it under
+// BATCH_FRONTIER), so lines fill in L2 and leave whole.  A batch's vectors one after the other.
 template<uint32_t SW>
 __global__ void __launch_bounds__(256)
 partition_kernel(const Config cfg, uint32_t lg_bins, const uint32_t* scalars, uint32_t* bin_cur, uint2* staging)
 {
     const uint32_t lane = threadIdx.x & 31;
-    for (uint32_t i0 = blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < cfg.npoints; i0 += gridDim.x * blockDim.x) {
-        const uint32_t i = i0 + lane;
-        for_each_digit<SW>(cfg, lg_bins, scalars, i, i < cfg.npoints, digit_count(cfg),
-                       [&](uint32_t w, bool nz, uint32_t bin, uint32_t b, uint32_t entry) {
-            const uint32_t peers = __match_any_sync(0xffffffffu, nz ? bin : ~0u);
-            const uint32_t leader = __ffs(peers) - 1;
-            uint32_t pos = 0;
-            if (nz && lane == leader) pos = atomicAdd(&bin_cur[bin], __popc(peers));
-            pos = __shfl_sync(0xffffffffu, pos, leader) + __popc(peers & ((1u << lane) - 1));
-            if (nz) staging[(size_t)w * row_stride(cfg) + pos] = make_uint2(entry, b);
-        });
-    }
+    for (uint32_t g = 0; g < cfg.nvecs; g++)
+        for (uint32_t i0 = blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < cfg.npoints; i0 += gridDim.x * blockDim.x) {
+            const uint32_t i = i0 + lane;
+            for_each_digit<SW>(cfg, lg_bins, scalars, i, i < cfg.npoints, digit_count(cfg),
+                           [&](uint32_t w, bool nz, uint32_t bin, uint32_t b, uint32_t entry) {
+                const uint32_t peers = __match_any_sync(0xffffffffu, nz ? bin : ~0u);
+                const uint32_t leader = __ffs(peers) - 1;
+                uint32_t pos = 0;
+                if (nz && lane == leader) pos = atomicAdd(&bin_cur[bin], __popc(peers));
+                pos = __shfl_sync(0xffffffffu, pos, leader) + __popc(peers & ((1u << lane) - 1));
+                if (nz) staging[(size_t)w * row_stride(cfg) + pos] = make_uint2(entry, b);
+            }, g);
+        }
 }
 
 // pass 3: one CTA per bin (blockIdx.x = w << lg_bins | bin).  Bucket histogram of the bin in
@@ -630,19 +637,24 @@ combine_par_kernel(const uint32_t* inR, const uint32_t* inS, uint32_t G, uint32_
     }
 }
 
+// one CTA per vector of the group: CTA b folds the V window sums of sets [bV, bV + V) into the
+// Jacobian point b of out_jacobian
 template<class F>
 __global__ void __launch_bounds__(32)
 finish_par_kernel(const Config cfg, const uint32_t* winR, uint32_t* out_jacobian)
 {
     __shared__ F slots[Par4<F>::NS];
     if (threadIdx.x >= 4) return;
+    const uint32_t V = vec_sets(cfg);
+    winR += (size_t)blockIdx.x * V * 4 * F::N;
+    out_jacobian += (size_t)blockIdx.x * 3 * F::N;
     Par4<F> p(slots, slots + 4, threadIdx.x);
     {
-        const ec::xyzz_t<F> top = load_bucket<F>(winR, cfg.nwins - 1);
+        const ec::xyzz_t<F> top = load_bucket<F>(winR, V - 1);
         if (p.lane == 0) { slots[Par4<F>::sX] = top.X; slots[Par4<F>::sY] = top.Y; slots[Par4<F>::sZZZ] = top.ZZZ; slots[Par4<F>::sZZ] = top.ZZ; }
         p.sync();
     }
-    for (uint32_t w = cfg.nwins - 1; w-- > 0;) {
+    for (uint32_t w = V - 1; w-- > 0;) {
         for (uint32_t d = 0; d < cfg.wbits; d++) p.dbl();
         p.add(load_bucket<F>(winR, w));
     }
@@ -751,10 +763,57 @@ public:
         return begin(make_config(total_points, nbits, scalar_bytes), slice_cap, stream);
     }
 
-    // a given geometry (make_config, or config_for_table for the rows of a precomputed table)
+    // a given geometry (make_config, or config_for_table for the rows of a precomputed table; a batch's
+    // group_config of either)
     Job begin(const Config& cfg, size_t slice_cap, cudaStream_t stream)
     {
         Job j;
+        CUDA_OK(cudaMallocAsync((void**)&j.blob, plan(j, cfg, slice_cap, nullptr), stream));
+        j.owner = stream;
+        plan(j, cfg, slice_cap, j.blob);
+        g_profile.reset();
+        return j;
+    }
+
+    // device scratch of a job of geometry cfg over slices of slice_cap points
+    static size_t scratch_bytes(const Config& cfg, size_t slice_cap)
+    {
+        Job j;
+        return plan(j, cfg, slice_cap, nullptr);
+    }
+
+    // ---- batches: G vectors per job (Config::nvecs), the groups of a batch one after the other -------
+    // A group's scratch is G times one vector's (staging, sorted, buckets, running sums: all of it
+    // scales with the sets), and its partition keeps G V 2^lg_bins bins open.  G is the largest count
+    // that keeps
+    //   - the scratch within BATCH_SCRATCH (2 GiB: 5 vectors of 2^20 BLS12-381 G1 points, 39 of 2^16)
+    //   - the partition's write frontier G V 2^lg_bins * 128 B within BATCH_FRONTIER (24 MB, under half
+    //     of the H100's 50 MB L2, as one vector's 13.6 MB at 2^26 points; 256 KB per vector at 2^20)
+    // with the batch then spread evenly over the groups that takes.  G = 1 from BATCH_MAX_POINTS points
+    // on: batches were measured faster than a loop of single calls at every shape up to 2^20 points
+    // (x1.25 to x20 on an H100 SXM at 700 W, DESIGN.md section 5d), larger ones were not measured.
+    // SPPARK_B200_MSM_BATCH_GROUP forces G (tests).
+    static constexpr size_t BATCH_SCRATCH = (size_t)2 << 30, BATCH_FRONTIER = (size_t)24 << 20;
+    static constexpr size_t BATCH_MAX_POINTS = (size_t)1 << 21;
+    static uint32_t group_size(const Config& cfg1, size_t slice_cap, size_t batch)
+    {
+        if (const char* env = getenv("SPPARK_B200_MSM_BATCH_GROUP"))
+            if (atoi(env) > 0) return (uint32_t)std::min<size_t>(batch, (size_t)atoi(env));
+        if (batch <= 1 || cfg1.npoints >= BATCH_MAX_POINTS) return 1;
+        Config c1 = cfg1;
+        c1.npoints = (uint32_t)slice_cap;
+        const size_t frontier = ((size_t)c1.nwins << sort_lg_bins(c1, row_stride(c1))) * 128;
+        const size_t g = std::min(BATCH_SCRATCH / scratch_bytes(cfg1, slice_cap), BATCH_FRONTIER / frontier);
+        // the bucket slots and bins of a group are counted in 32 bits
+        const size_t g_slots = ((size_t)1 << 31) / ((size_t)cfg1.nwins << cfg1.lg_nb);
+        const size_t gmax = std::max<size_t>(1, std::min({g, g_slots, batch})), ngroups = (batch + gmax - 1) / gmax;
+        return (uint32_t)((batch + ngroups - 1) / ngroups);
+    }
+
+private:
+    // the scratch of a job in one blob: j's geometry and, with a blob, its pointers; returns the bytes
+    static size_t plan(Job& j, const Config& cfg, size_t slice_cap, uint8_t* blob)
+    {
         j.cfg = cfg;
         j.cfg.npoints = (uint32_t)slice_cap;
         j.slice_cap = slice_cap;
@@ -791,21 +850,20 @@ public:
             o_pre = take((size_t)j.pair_threads * PAIR_K * F::N * 4);
             o_tot = take((size_t)j.pair_threads * F::N * 4);
         }
-        CUDA_OK(cudaMallocAsync((void**)&j.blob, off, stream));
-        j.owner = stream;
-        auto U32 = [&](size_t o) { return reinterpret_cast<uint32_t*>(j.blob + o); };
+        if (!blob) return off;
+        auto U32 = [&](size_t o) { return reinterpret_cast<uint32_t*>(blob + o); };
         j.counts = U32(o_counts); j.offsets = U32(o_offsets); j.cursor = U32(o_cursor);
         j.ctrl = U32(o_ctrl); j.heavy_list = U32(o_heavy); j.chunk_map = U32(o_cmap);
         j.partials = U32(o_partials); j.sorted = U32(o_sorted); j.buckets = U32(o_buckets);
         j.bin_count = U32(o_bcount); j.bin_base = U32(o_bbase); j.bin_cur = U32(o_bcur); j.overflow = U32(o_over);
-        j.staging = reinterpret_cast<uint2*>(j.blob + o_staging);
+        j.staging = reinterpret_cast<uint2*>(blob + o_staging);
         j.R[0] = U32(o_r0); j.S[0] = U32(o_s0); j.R[1] = U32(o_r1); j.S[1] = U32(o_s1);
         j.counts1 = U32(o_c1); j.off1 = U32(o_o1); j.wintotal = U32(o_wt); j.winbase = U32(o_wb);
         j.sums = U32(o_sums); j.pre = U32(o_pre); j.totals = U32(o_tot);
-        g_profile.reset();
-        return j;
+        return off;
     }
 
+public:
     // fold `n` (<= slice_cap) device-resident points/scalars into the buckets
     void slice(Job& j, const uint32_t* d_points, const uint32_t* d_scalars, size_t n, cudaStream_t stream)
     {
@@ -866,18 +924,18 @@ public:
             CUDA_OK(cudaMemcpyAsync(dbg, j.ctrl, 12, cudaMemcpyDeviceToHost, stream));
             CUDA_OK(cudaStreamSynchronize(stream));
             fprintf(stderr, "[msm] slice %u n=%u wbits=%u nwins=%u heavy_thr=%u tasks_claimed=%u nheavy=%u nchunks=%u acc_blocks=%u"
-                    " digits=%u sets=%u copies=%u nbits=%u sbytes=%u\n",
+                    " digits=%u sets=%u copies=%u nbits=%u sbytes=%u vecs=%u vsets=%u\n",
                     j.slices_done, cfg.npoints, cfg.wbits, cfg.nwins, cfg.heavy, dbg[0], dbg[1], dbg[2], acc_blocks,
-                    digit_count(cfg), cfg.nwins, cfg.copies, (uint32_t)cfg.nbits, 4u * cfg.swords);
+                    digit_count(cfg), cfg.nwins, cfg.copies, (uint32_t)cfg.nbits, 4u * cfg.swords, cfg.nvecs, vec_sets(cfg));
         }
         j.slices_done++;
     }
 
-    // running sums over the buckets, Horner over the windows -> d_out (JW words), frees the job
+    // running sums over the buckets, Horner over the windows -> d_out (JW words per vector), frees the job
     void finish(Job& j, uint32_t* d_out, cudaStream_t stream)
     {
         if (j.slices_done == 0) {
-            CUDA_OK(cudaMemsetAsync(d_out, 0, JW * 4, stream));
+            CUDA_OK(cudaMemsetAsync(d_out, 0, (size_t)j.cfg.nvecs * JW * 4, stream));
         } else {
             const Config& cfg = j.cfg;
             g_profile.mark("reduce", stream);
@@ -897,7 +955,7 @@ public:
                 cur ^= 1;
             }
             g_profile.mark("finish", stream);
-            finish_par_kernel<F><<<1, 32, 0, stream>>>(cfg, j.R[cur], d_out);
+            finish_par_kernel<F><<<cfg.nvecs, 32, 0, stream>>>(cfg, j.R[cur], d_out);
             COUNT_LAUNCH();
             g_profile.mark("end", stream);
             CUDA_OK(cudaGetLastError());
@@ -906,18 +964,27 @@ public:
         j.blob = nullptr;
     }
 
-    // all inputs device-resident: d_points packed affine, d_scalars scalar_bytes each (bits from nbits
-    // up ignored).  d_out: JW words of device memory.  Enqueues on `stream`; no synchronisation.
+    // all inputs device-resident: d_points packed affine, d_scalars `batch` vectors of npoints scalars of
+    // scalar_bytes each (bits from nbits up ignored), run in groups of group_size vectors.  d_out: batch
+    // * JW words of device memory.  Enqueues on `stream`; no synchronisation.
     void invoke_dev(uint32_t* d_out, const uint32_t* d_points, size_t npoints,
-                    const uint32_t* d_scalars, cudaStream_t stream, uint32_t nbits = 255, uint32_t scalar_bytes = 32)
+                    const uint32_t* d_scalars, cudaStream_t stream, uint32_t nbits = 255, uint32_t scalar_bytes = 32,
+                    size_t batch = 1)
     {
         if (npoints == 0) {
-            CUDA_OK(cudaMemsetAsync(d_out, 0, JW * 4, stream));
+            CUDA_OK(cudaMemsetAsync(d_out, 0, batch * JW * 4, stream));
             return;
         }
-        Job j = begin(npoints, npoints, stream, nbits, scalar_bytes);
-        slice(j, d_points, d_scalars, npoints, stream);
-        finish(j, d_out, stream);
+        if (npoints >= (1ull << 31))
+            throw cuda_error(-(int)cudaErrorInvalidValue, "msm: npoints must be < 2^31");
+        const Config cfg1 = make_config(npoints, nbits, scalar_bytes);
+        const size_t G = group_size(cfg1, npoints, batch), sw = scalar_bytes / 4;
+        for (size_t b0 = 0; b0 < batch; b0 += G) {
+            const uint32_t g = (uint32_t)std::min(G, batch - b0);
+            Job j = begin(group_config(cfg1, g), npoints, stream);
+            slice(j, d_points, d_scalars + b0 * npoints * sw, npoints, stream);
+            finish(j, d_out + b0 * JW, stream);
+        }
     }
 };
 

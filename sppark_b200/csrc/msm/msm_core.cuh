@@ -29,9 +29,15 @@ namespace msm {
 // of copy k, so V = ceil(D / K) bucket sets and V - 1 Horner steps cover all D digits.  With one
 // copy the digit count D and the bucket-set count are both nwins; everything below loops over
 // the bucket sets ("windows") as before.
+//
+// Batches (nvecs = G > 1): G scalar vectors against the same points, one after the other in the scalar
+// array (vector g's scalars start g * npoints * swords words after vector 0).  Each vector has its own
+// V = nwins / G bucket sets: set s belongs to vector s / V, and vector g's digit w goes to set
+// g V + digit_slot(w).  The bucket entry stays point | sign << 31, since the points are shared, and the
+// kernels after the sort see nwins sets as for one vector.
 struct Config {
     uint32_t wbits;        // c: window width
-    uint32_t nwins;        // bucket sets V: D = ceil((nbits + 1) / c) without a table, ceil(D / K) with one
+    uint32_t nwins;        // bucket sets G V; per vector V: D = ceil((nbits + 1) / c) without a table, ceil(D / K) with one
     uint32_t lg_nb;        // c - 1: log2(buckets per window)
     uint32_t npoints;
     uint32_t heavy;        // buckets with more entries go to the cooperative kernel
@@ -44,7 +50,18 @@ struct Config {
     // the struct's padding, so the kernel parameters after a Config keep their offsets.
     uint16_t nbits;        // 1 .. min(255, 32 * swords)
     uint16_t swords;       // 32-bit words per scalar: 1, 2, 4 or 8
+    uint32_t nvecs;        // G: scalar vectors of the group (1 without a batch)
 };
+
+// V: the bucket sets of one vector
+HD uint32_t vec_sets(const Config& cfg) { return cfg.nvecs == 1 ? cfg.nwins : cfg.nwins / cfg.nvecs; }
+// the geometry of G vectors, each with the sets of the one-vector geometry cfg
+inline Config group_config(Config cfg, uint32_t nvecs)
+{
+    cfg.nwins *= nvecs;
+    cfg.nvecs = nvecs;
+    return cfg;
+}
 
 // digits per scalar, D = ceil((nbits + 1) / c) (equal to nwins without a table): the top digit never
 // carries out of the last window; ceil(256 / c) for 255-bit scalars
@@ -54,13 +71,14 @@ HD uint32_t digit_count(const Config& cfg) { return digits_for(cfg.nbits, cfg.wb
 // (a 32-bit product: a table keeps copies * points < 2^31, the bucket entry's index range)
 HD size_t row_stride(const Config& cfg) { return cfg.copies * cfg.npoints; }
 
-// digit w of point i -> bucket set v = w mod V (returned) and entry (i + (w / V) * copy_stride) | sign << 31
+// digit w of point i -> bucket set v = w mod V of its vector (returned) and entry
+// (i + (w / V) * copy_stride) | sign << 31
 HD uint32_t digit_slot(const Config& cfg, uint32_t w, uint32_t i, uint32_t neg, uint32_t& entry)
 {
     if (cfg.copies == 1) { entry = i | (neg << 31); return w; }
-    const uint32_t k = w / cfg.nwins;
+    const uint32_t V = vec_sets(cfg), k = w / V;
     entry = (i + k * cfg.copy_stride) | (neg << 31);
-    return w - k * cfg.nwins;
+    return w - k * V;
 }
 
 HD uint32_t atomic_inc(uint32_t* p, uint32_t v = 1)
@@ -130,11 +148,15 @@ struct Digits {
     }
 };
 
-// fn(Digits<swords>&) for scalar i of a scalar array in the format of cfg (host-side bodies: the
-// device kernels are instantiated per width instead)
+// first scalar word of vector g
+HD size_t vec_offset(const Config& cfg, uint32_t g) { return (size_t)g * cfg.npoints * cfg.swords; }
+
+// fn(Digits<swords>&) for scalar i of vector g of a scalar array in the format of cfg (host-side bodies:
+// the device kernels are instantiated per width instead)
 template<class Fn>
-HD void with_digits(const Config& cfg, const uint32_t* scalars, uint32_t i, Fn fn)
+HD void with_digits(const Config& cfg, const uint32_t* scalars, uint32_t i, Fn fn, uint32_t g = 0)
 {
+    scalars += vec_offset(cfg, g);
     switch (cfg.swords) {
     case 1: { Digits<1> d(scalars + (size_t)i, cfg.nbits); fn(d); break; }
     case 2: { Digits<2> d(scalars + 2 * (size_t)i, cfg.nbits); fn(d); break; }
@@ -149,32 +171,35 @@ HD void with_digits(const Config& cfg, const uint32_t* scalars, uint32_t i, Fn f
 // (up to the order inside a bucket), and the CPU single-stepper of the whole pipeline
 // (tests/emu/msm_emu.cpp) runs it.  The device does not: with 2^(c-1) buckets per window its
 // random 4-byte stores keep more partly written lines open than L2 holds.
-HD void count_body(const Config& cfg, const uint32_t* scalars, uint32_t* counts, uint32_t i)
+// g: the vector of a batch (Config::nvecs) whose scalar i is counted / placed
+HD void count_body(const Config& cfg, const uint32_t* scalars, uint32_t* counts, uint32_t i, uint32_t g = 0)
 {
+    const uint32_t s0 = g * vec_sets(cfg);
     with_digits(cfg, scalars, i, [&](auto& d) {
         const uint32_t nd = digit_count(cfg);
         for (uint32_t w = 0; w < nd; w++) {
             uint32_t b, neg, entry;
             if (d.next(w, cfg.wbits, b, neg))
-                atomic_inc(&counts[((size_t)digit_slot(cfg, w, i, neg, entry) << cfg.lg_nb) + b]);
+                atomic_inc(&counts[((size_t)(s0 + digit_slot(cfg, w, i, neg, entry)) << cfg.lg_nb) + b]);
         }
-    });
+    }, g);
 }
 
 // digits [w0, w1) only: digits below w0 are still walked for their carry
 HD void scatter_body(const Config& cfg, const uint32_t* scalars, uint32_t* cursor,
-                     uint32_t* sorted, uint32_t i, uint32_t w0, uint32_t w1)
+                     uint32_t* sorted, uint32_t i, uint32_t w0, uint32_t w1, uint32_t g = 0)
 {
+    const uint32_t s0 = g * vec_sets(cfg);
     with_digits(cfg, scalars, i, [&](auto& d) {
         for (uint32_t w = 0; w < w1; w++) {
             uint32_t b, neg, entry;
             if (d.next(w, cfg.wbits, b, neg) && w >= w0) {
-                const uint32_t v = digit_slot(cfg, w, i, neg, entry);
+                const uint32_t v = s0 + digit_slot(cfg, w, i, neg, entry);
                 uint32_t pos = atomic_inc(&cursor[((size_t)v << cfg.lg_nb) + b]);
                 sorted[(size_t)v * row_stride(cfg) + pos] = entry;
             }
         }
-    });
+    }, g);
 }
 
 // ---- sort: (window, bucket) lists of point indices -----------------------------------------
@@ -195,16 +220,18 @@ constexpr uint32_t SORT_LG_FILL = 13;   // bins hold about 2^13 entries of a uni
 // c divides nbits and the window holds only the carry)
 HD uint32_t top_window_bits(const Config& cfg)
 {
-    const uint32_t e = cfg.nbits - (cfg.nwins - 1) * cfg.wbits;
+    const uint32_t e = cfg.nbits - (vec_sets(cfg) - 1) * cfg.wbits;
     return e < cfg.lg_nb ? e : cfg.lg_nb;
 }
-// with a table the thin top digit shares its bucket set with full-width digits: every set is full
-HD uint32_t window_bits(const Config& cfg, uint32_t w)
-{   return w + 1 < cfg.nwins || cfg.copies > 1 ? cfg.lg_nb : top_window_bits(cfg);   }
-// buckets per bin of window w: 2^s_w, so the window's used buckets [0, 2^ub) make <= 2^lg_bins bins
-HD uint32_t bin_shift(const Config& cfg, uint32_t lg_bins, uint32_t w)
+// with a table the thin top digit shares its bucket set with full-width digits: every set is full.
+// v: the set's index inside its vector (w mod V for set w)
+HD uint32_t window_bits(const Config& cfg, uint32_t v)
+{   return v + 1 < vec_sets(cfg) || cfg.copies > 1 ? cfg.lg_nb : top_window_bits(cfg);   }
+// buckets per bin of a window with vector-local index v: 2^s_v, so the window's used buckets [0, 2^ub)
+// make <= 2^lg_bins bins
+HD uint32_t bin_shift(const Config& cfg, uint32_t lg_bins, uint32_t v)
 {
-    const uint32_t ub = window_bits(cfg, w);
+    const uint32_t ub = window_bits(cfg, v);
     return ub > lg_bins ? ub - lg_bins : 0;
 }
 
@@ -224,7 +251,7 @@ inline uint32_t sort_lg_bins(const Config& cfg, size_t n)
 // window's used buckets (always empty)
 HD bool bin_buckets(const Config& cfg, uint32_t lg_bins, uint32_t w, uint32_t bin, uint32_t& b0, uint32_t& nbk)
 {
-    const uint32_t s = bin_shift(cfg, lg_bins, w), ub = window_bits(cfg, w);
+    const uint32_t v = w % vec_sets(cfg), s = bin_shift(cfg, lg_bins, v), ub = window_bits(cfg, v);
     b0 = bin << s;
     nbk = 1u << s;
     return b0 < (1u << ub);
@@ -232,22 +259,29 @@ HD bool bin_buckets(const Config& cfg, uint32_t lg_bins, uint32_t w, uint32_t bi
 
 // the last used bin of a window also owns the offsets of the never-used buckets above it
 HD bool last_bin(const Config& cfg, uint32_t lg_bins, uint32_t w, uint32_t bin)
-{   return ((bin + 1) << bin_shift(cfg, lg_bins, w)) == (1u << window_bits(cfg, w));   }
+{
+    const uint32_t v = w % vec_sets(cfg);
+    return ((bin + 1) << bin_shift(cfg, lg_bins, v)) == (1u << window_bits(cfg, v));
+}
 
-// every digit of point i in order: fn(set, nonzero, bin (global), bucket, entry), with set and entry
-// from digit_slot (without a table: set = digit index, entry = i | sign << 31).  Digits >= w_end are
-// not visited.  `valid` false: fn sees only zero digits (the tail lanes of a warp that must still
-// take part in its collective operations).  SW: cfg.swords, the scalar width the kernel is built for.
+// every digit of point i of vector g in order: fn(set, nonzero, bin (global), bucket, entry), with set
+// g V + v and entry from digit_slot (without a table and batch: set = digit index, entry = i | sign << 31).
+// Digits >= w_end are not visited.  `valid` false: fn sees only zero digits (the tail lanes of a warp
+// that must still take part in its collective operations).  SW: cfg.swords, the scalar width the
+// kernel is built for.
 template<uint32_t SW = 8, class Fn>
 HD void for_each_digit(const Config& cfg, uint32_t lg_bins, const uint32_t* scalars, uint32_t i, bool valid,
-                       uint32_t w_end, Fn fn)
+                       uint32_t w_end, Fn fn, uint32_t g = 0)
 {
-    Digits<SW> d(scalars + SW * (size_t)(valid ? i : 0), cfg.nbits);
+    Digits<SW> d(scalars + (size_t)g * cfg.npoints * SW + SW * (size_t)(valid ? i : 0), cfg.nbits);
+    const uint32_t V = vec_sets(cfg), s0 = g * V;
+    // bin_shift of the vector's top set and of the others, once per scalar
+    const uint32_t top = bin_shift(cfg, lg_bins, V - 1), full = bin_shift(cfg, lg_bins, 0);
     for (uint32_t w = 0; w < w_end; w++) {
         uint32_t b, neg, entry;
         const bool nz = d.next(w, cfg.wbits, b, neg) && valid;
-        const uint32_t v = digit_slot(cfg, w, i, neg, entry);
-        fn(v, nz, (v << lg_bins) + (nz ? b >> bin_shift(cfg, lg_bins, v) : 0), b, entry);
+        const uint32_t v = digit_slot(cfg, w, i, neg, entry), s = s0 + v;
+        fn(s, nz, (s << lg_bins) + (nz ? b >> (v + 1 < V ? full : top) : 0), b, entry);
     }
 }
 
@@ -418,13 +452,15 @@ HD void combine_body(const uint32_t* inR, const uint32_t* inS, uint32_t G, uint3
     store_bucket<F>(outS, item, acc);
 }
 
-// finish: out = sum_w 2^(c*w) * R_w over the nwins bucket sets, as a Jacobian point with canonical
-// coordinates (with a table, set v holds every digit v + kV, its factor 2^(cVk) already in the points)
+// finish: out = sum_w 2^(c*w) * R_w over the V bucket sets of one vector, as a Jacobian point with
+// canonical coordinates (with a table, set v holds every digit v + kV, its factor 2^(cVk) already in
+// the points).  winR: the vector's first set; a batch's vector g reads from set g V on.
 template<class F>
 HD void finish_body(const Config& cfg, const uint32_t* winR, uint32_t* out_jacobian)
 {
-    ec::xyzz_t<F> acc = load_bucket<F>(winR, cfg.nwins - 1);
-    for (uint32_t w = cfg.nwins - 1; w-- > 0;) {
+    const uint32_t V = vec_sets(cfg);
+    ec::xyzz_t<F> acc = load_bucket<F>(winR, V - 1);
+    for (uint32_t w = V - 1; w-- > 0;) {
         for (uint32_t d = 0; d < cfg.wbits; d++) acc.dbl_hot();
         acc.add_hot(load_bucket<F>(winR, w));
     }
@@ -491,6 +527,7 @@ inline Config make_config(size_t npoints, uint32_t nbits, uint32_t scalar_bytes)
     cfg.copy_stride = (uint32_t)npoints;
     cfg.nbits = (uint16_t)nbits;
     cfg.swords = (uint16_t)(scalar_bytes / 4);
+    cfg.nvecs = 1;
     set_heavy(cfg, (uint64_t)cfg.nwins * npoints);
     return cfg;
 }
@@ -518,6 +555,7 @@ inline Config config_for_table(size_t n, uint32_t wbits, uint32_t copies, size_t
     cfg.copy_stride = (uint32_t)stride;
     cfg.nbits = (uint16_t)nbits;
     cfg.swords = (uint16_t)(scalar_bytes / 4);
+    cfg.nvecs = 1;
     set_heavy(cfg, (uint64_t)Db * n);
     return cfg;
 }

@@ -44,16 +44,21 @@ void scalars_from_mont(uint32_t* d_scalars, size_t n, cudaStream_t stream)
 // `table` (with `resident`): the rows are a precomputed table of that width and copy count, whose
 // copies lie table->copy_stride rows apart; slice k's points start at row `first` of every copy.
 // scalar_bytes / nbits: the scalar format (msm_core.cuh Config); each slice uploads n * scalar_bytes.
+// batch: vectors of npoints scalars one after the other, out one Jacobian point per vector.  They run
+// in groups of msm_t::group_size vectors (Config::nvecs), each group sliced as one vector is: slice k
+// of group q uploads its G rows of scalars on the copy stream while the unit before it computes.
 template<class F, class Fr>
 RustError msm_slices(void* out, const void* points, size_t npoints, const void* scalars, size_t stride,
                      bool has_flag, bool mont, const uint32_t* resident, const msm::Config* table,
-                     uint32_t scalar_bytes, uint32_t nbits)
+                     uint32_t scalar_bytes, uint32_t nbits, size_t batch = 1)
 {
     constexpr size_t PB = 2 * F::N * 4, JB = 3 * F::N * 4;
     try {
         const gpu_t& gpu = select_gpu(-1);
         gpu.select();
-        if (npoints == 0) { memset(out, 0, JB); return rust_ok(); }
+        if (npoints == 0) { memset(out, 0, batch * JB); return rust_ok(); }
+        if (npoints >= (1ull << 31))
+            throw cuda_error(-(int)cudaErrorInvalidValue, "msm: npoints must be < 2^31");
         if (!resident && stride < PB + (has_flag ? 1 : 0))
             return rust_err(-(int)cudaErrorInvalidValue, "msm: affine stride too small");
         if (!resident && stride % 4 != 0)        // rows are packed on the device with 32-bit loads
@@ -101,8 +106,13 @@ RustError msm_slices(void* out, const void* points, size_t npoints, const void* 
         } else {
             sched.push_back(npoints);
         }
-        const size_t nslices = sched.size(), nbuf = nslices > 1 ? 2 : 1;
+        const size_t nslices = sched.size();
         const size_t slice_n = *std::max_element(sched.begin(), sched.end());
+        const msm::Config cfg1 = table ? msm::config_for_table(npoints, table->wbits, table->copies, table->copy_stride,
+                                                               nbits, scalar_bytes)
+                                       : msm::make_config(npoints, nbits, scalar_bytes);
+        const size_t G = msm::msm_t<F>::group_size(cfg1, slice_n, batch);
+        const size_t nunits = (batch + G - 1) / G * nslices, nbuf = nunits > 1 ? 2 : 1;
         const bool pageable = (!resident && stager_t::is_pageable(points)) || stager_t::is_pageable(scalars);
         std::unique_lock<std::mutex> stage_lock(gpu.stage_mtx, std::defer_lock);
         if (pageable) stage_lock.lock();
@@ -111,9 +121,9 @@ RustError msm_slices(void* out, const void* points, size_t npoints, const void* 
             else copy.HtoD(dst, src, bytes);
         };
 
-        dev_ptr_t<uint32_t> d_out(JB / 4, compute);
+        dev_ptr_t<uint32_t> d_out(batch * JB / 4, compute);
         const size_t SW = scalar_bytes / 4;                        // 32-bit words per scalar
-        dev_ptr_t<uint32_t> d_points(resident ? 1 : nbuf * slice_n * (PB / 4), compute), d_scalars(nbuf * slice_n * SW, compute);
+        dev_ptr_t<uint32_t> d_points(resident ? 1 : nbuf * slice_n * (PB / 4), compute), d_scalars(nbuf * G * slice_n * SW, compute);
         dev_ptr_t<uint8_t> d_raw(packed ? 1 : nbuf * slice_n * stride, compute);
         event_t copied[2], consumed[2], ready;
         ready.record(compute);                                    // buffers exist
@@ -128,45 +138,48 @@ RustError msm_slices(void* out, const void* points, size_t npoints, const void* 
         } drain{compute, copy};
 
         msm::msm_t<F> m(gpu);
-        auto job = table ? m.begin(msm::config_for_table(npoints, table->wbits, table->copies, table->copy_stride,
-                                                         nbits, scalar_bytes),
-                                   slice_n, compute)
-                         : m.begin(npoints, slice_n, compute, nbits, scalar_bytes);
-        size_t first = 0;
-        for (size_t k = 0; k < nslices; first += sched[k], k++) {
-            const size_t b = k & (nbuf - 1), n = sched[k];
-            const uint32_t* dp = resident ? resident + first * (PB / 4) : d_points + b * slice_n * (PB / 4);
-            uint32_t* ds = d_scalars + b * slice_n * SW;
-            if (k >= nbuf) consumed[b].wait(copy);                                // buffer free again
-            upload(ds, (const uint8_t*)scalars + first * scalar_bytes, n * scalar_bytes);
-            if (resident) {
-            } else if (packed) {
-                upload(d_points + b * slice_n * (PB / 4), (const uint8_t*)points + first * PB, n * PB);
-            } else {
-                uint8_t* dr = d_raw + b * slice_n * stride;
-                upload(dr, (const uint8_t*)points + first * stride, n * stride);
-                uint32_t blocks = (uint32_t)std::min<size_t>((n + 255) / 256, (size_t)gpu.sm_count() * 8);
-                msm::pack_points_kernel<<<blocks, 256, 0, copy>>>(dr, stride, PB / 4, has_flag,
-                                                                  d_points + b * slice_n * (PB / 4), (uint32_t)n);
-                COUNT_LAUNCH();
-                CUDA_OK(cudaGetLastError());
+        for (size_t v0 = 0, u = 0; v0 < batch; v0 += G) {
+            const uint32_t g = (uint32_t)std::min(G, batch - v0);
+            auto job = m.begin(msm::group_config(cfg1, g), slice_n, compute);
+            size_t first = 0;
+            for (size_t k = 0; k < nslices; first += sched[k], k++, u++) {
+                const size_t b = u & (nbuf - 1), n = sched[k];
+                const uint32_t* dp = resident ? resident + first * (PB / 4) : d_points + b * slice_n * (PB / 4);
+                uint32_t* ds = d_scalars + b * G * slice_n * SW;
+                if (u >= nbuf) consumed[b].wait(copy);                                // buffer free again
+                // vector v0 + r of the group: its n scalars from `first` on, as row r of the buffer
+                const uint8_t* src = (const uint8_t*)scalars + (v0 * npoints + first) * scalar_bytes;
+                if (n == npoints) upload(ds, src, g * n * scalar_bytes);
+                else for (uint32_t r = 0; r < g; r++) upload(ds + r * n * SW, src + r * npoints * scalar_bytes, n * scalar_bytes);
+                if (resident) {
+                } else if (packed) {
+                    upload(d_points + b * slice_n * (PB / 4), (const uint8_t*)points + first * PB, n * PB);
+                } else {
+                    uint8_t* dr = d_raw + b * slice_n * stride;
+                    upload(dr, (const uint8_t*)points + first * stride, n * stride);
+                    uint32_t blocks = (uint32_t)std::min<size_t>((n + 255) / 256, (size_t)gpu.sm_count() * 8);
+                    msm::pack_points_kernel<<<blocks, 256, 0, copy>>>(dr, stride, PB / 4, has_flag,
+                                                                      d_points + b * slice_n * (PB / 4), (uint32_t)n);
+                    COUNT_LAUNCH();
+                    CUDA_OK(cudaGetLastError());
+                }
+                copied[b].record(copy);
+                copied[b].wait(compute);
+                if (mont) scalars_from_mont<Fr>(ds, g * n, compute);
+                m.slice(job, dp, ds, n, compute);
+                consumed[b].record(compute);
             }
-            copied[b].record(copy);
-            copied[b].wait(compute);
-            if (mont) scalars_from_mont<Fr>(ds, n, compute);
-            m.slice(job, dp, ds, n, compute);
-            consumed[b].record(compute);
+            m.finish(job, d_out + v0 * (JB / 4), compute);
         }
-        m.finish(job, d_out, compute);
-        compute.DtoH(out, d_out, JB);
+        compute.DtoH(out, d_out, batch * JB);
         compute.sync();
         copy.sync();
         drain.armed = false;
     } catch (const cuda_error& e) {
-        memset(out, 0, JB);                      // out->inf(), as the reference does on failure
+        memset(out, 0, batch * JB);              // out->inf(), as the reference does on failure
         return rust_err(e.code(), e.what());
     } catch (const std::exception& e) {
-        memset(out, 0, JB);
+        memset(out, 0, batch * JB);
         return rust_err(-1, e.what());
     }
     return rust_ok();
@@ -198,7 +211,7 @@ RustError msm_preload(const void* points, size_t npoints, size_t stride, bool ha
         if (stride % 4 != 0)
             return rust_err(-(int)cudaErrorInvalidValue, "msm: affine stride must be a multiple of 4 bytes");
         if (npoints >= (1ull << 31))
-            return rust_err(-(int)cudaErrorInvalidValue, "msm: npoints must be < 2^31");
+            throw cuda_error(-(int)cudaErrorInvalidValue, "msm: npoints must be < 2^31");
         const uint32_t want = copies ? *copies : 1;
         if (want == 0)
             return rust_err(-(int)cudaErrorInvalidValue, "msm: a precomputed table needs at least one copy");
@@ -248,41 +261,58 @@ RustError msm_preload(const void* points, size_t npoints, size_t stride, bool ha
 // MSM of host scalars against the first npoints rows of a msm_preload buffer; wbits / copies /
 // copy_stride: the table it holds (copies = 1: plain rows, the window width follows npoints and the
 // scalar format)
+// batch: vectors of npoints host scalars one after the other (msm_slices), out one point per vector
+template<class F, class Fr>
+RustError msm_resident_batch(void* out, const void* d_points, size_t npoints, const void* scalars, size_t batch,
+                             bool mont, uint32_t wbits, uint32_t copies, size_t copy_stride, uint32_t scalar_bytes,
+                             uint32_t nbits)
+{
+    if (copies <= 1)
+        return msm_slices<F, Fr>(out, nullptr, npoints, scalars, 0, false, mont, (const uint32_t*)d_points, nullptr,
+                                 scalar_bytes, nbits, batch);
+    const msm::Config table = msm::config_for_table(copy_stride, wbits, copies, copy_stride);
+    return msm_slices<F, Fr>(out, nullptr, npoints, scalars, 0, false, mont, (const uint32_t*)d_points, &table,
+                             scalar_bytes, nbits, batch);
+}
+
 template<class F, class Fr>
 RustError msm_resident(void* out, const void* d_points, size_t npoints, const void* scalars, bool mont,
                        uint32_t wbits, uint32_t copies, size_t copy_stride, uint32_t scalar_bytes, uint32_t nbits)
 {
-    if (copies <= 1)
-        return msm_slices<F, Fr>(out, nullptr, npoints, scalars, 0, false, mont, (const uint32_t*)d_points, nullptr,
-                                 scalar_bytes, nbits);
-    const msm::Config table = msm::config_for_table(copy_stride, wbits, copies, copy_stride);
-    return msm_slices<F, Fr>(out, nullptr, npoints, scalars, 0, false, mont, (const uint32_t*)d_points, &table,
-                             scalar_bytes, nbits);
+    return msm_resident_batch<F, Fr>(out, d_points, npoints, scalars, 1, mont, wbits, copies, copy_stride,
+                                     scalar_bytes, nbits);
 }
 
+// batch: vectors of npoints device scalars one after the other (msm_t::invoke_dev), out one point per vector
 template<class F>
-RustError msm_dev(void* out, const void* d_points, size_t npoints, const void* d_scalars, void* stream,
-                  uint32_t scalar_bytes, uint32_t nbits)
+RustError msm_dev_batch(void* out, const void* d_points, size_t npoints, const void* d_scalars, size_t batch,
+                        void* stream, uint32_t scalar_bytes, uint32_t nbits)
 {
     constexpr size_t JB = 3 * F::N * 4;
     try {
         const gpu_t& gpu = gpu_of_current_device();
         cudaStream_t s = (cudaStream_t)stream;
         const stream_t borrowed(s);
-        dev_ptr_t<uint32_t> d_out(JB / 4, borrowed);           // released on every exit path
+        dev_ptr_t<uint32_t> d_out(batch * JB / 4, borrowed);   // released on every exit path
         msm::msm_t<F> m(gpu);
-        m.invoke_dev(d_out, (const uint32_t*)d_points, npoints, (const uint32_t*)d_scalars, s, nbits, scalar_bytes);
-        CUDA_OK(cudaMemcpyAsync(out, d_out, JB, cudaMemcpyDeviceToHost, s));
+        m.invoke_dev(d_out, (const uint32_t*)d_points, npoints, (const uint32_t*)d_scalars, s, nbits, scalar_bytes,
+                     batch);
+        CUDA_OK(cudaMemcpyAsync(out, d_out, batch * JB, cudaMemcpyDeviceToHost, s));
         CUDA_OK(cudaStreamSynchronize(s));
     } catch (const cuda_error& e) {
-        memset(out, 0, JB);
+        memset(out, 0, batch * JB);
         return rust_err(e.code(), e.what());
     } catch (const std::exception& e) {
-        memset(out, 0, JB);
+        memset(out, 0, batch * JB);
         return rust_err(-1, e.what());
     }
     return rust_ok();
 }
+
+template<class F>
+RustError msm_dev(void* out, const void* d_points, size_t npoints, const void* d_scalars, void* stream,
+                  uint32_t scalar_bytes, uint32_t nbits)
+{   return msm_dev_batch<F>(out, d_points, npoints, d_scalars, 1, stream, scalar_bytes, nbits);   }
 
 
 // ---- synthetic inputs: out[i] = (i+1)*G, affine (role of util::generate_points_scalars,
@@ -364,7 +394,7 @@ constexpr curve_ops curve_row()
 {
     typedef typename G::F F;
     return {msm_host<F, Fr>, msm_dev<F>, gen_points<G>, combine<F>, msm_preload<F>, msm_resident<F, Fr>,
-            2 * F::N * 4, 3 * F::N * 4};
+            msm_resident_batch<F, Fr>, msm_dev_batch<F>, 2 * F::N * 4, 3 * F::N * 4};
 }
 
 }  // namespace

@@ -163,6 +163,21 @@ class MsmContext:
         _lib.check(err)
         return out
 
+    def invoke_batch(self, scalars, nbits=None):
+        """B scalar vectors against the preloaded points in one call: scalars (B, n, 4) or (B, n, 2)
+        uint64, or (B, n) uint64 or uint32, the width following the array as for msm() (plain
+        integers, bits from `nbits` up ignored).  Returns (B, 3 * limbs) uint64, row b the Jacobian
+        result of vector b.  The vectors share the sort, accumulate, reduce and finish launches
+        (DESIGN.md section 5d)."""
+        sbytes, B, n = _batch_format(scalars, np.uint64, np.uint32)
+        if not scalars.flags["C_CONTIGUOUS"]:
+            raise TypeError("scalars must be C-contiguous")
+        fmt = _scalar_format(sbytes, False, nbits) or (32, 255)
+        out = np.zeros((B, 3 * _LIMBS[self.curve]), dtype=np.uint64)
+        err = _lib.lib().sppark_b200_msm_ctx_invoke_batch(self._h, out.ctypes.data, scalars.ctypes.data, n, B, *fmt)
+        _lib.check(err)
+        return out
+
     def close(self):
         if self._h:
             _lib.lib().sppark_b200_msm_ctx_free(self._h)
@@ -199,6 +214,39 @@ def msm_dev(curve, d_points, d_scalars, npoints=None, stream=None, nbits=None):
         else:
             err = _lib.lib().sppark_b200_msm_dev_bits(curve, out.ctypes.data, d_points.data_ptr(), n,
                                                       d_scalars.data_ptr(), fmt[0], fmt[1], s)
+    _lib.check(err)
+    return out
+
+
+def _batch_format(scalars, u64, u32):
+    """(scalar_bytes, B, n) of a batch of B vectors of n scalars: (B, n, 4) / (B, n, 2) of 64-bit words,
+    (B, n) of 64- or 32-bit scalars"""
+    sbytes = None
+    if scalars.ndim == 3 and scalars.dtype == u64 and scalars.shape[2] in (2, 4):
+        sbytes = 8 * scalars.shape[2]
+    elif scalars.ndim == 2 and scalars.dtype in (u64, u32):
+        sbytes = 8 if scalars.dtype == u64 else 4
+    if sbytes is None:
+        raise TypeError("batched scalars must be (B, n, 4) or (B, n, 2) 64-bit words, or (B, n) of 64- or 32-bit "
+                        "scalars")
+    return sbytes, int(scalars.shape[0]), int(scalars.shape[1])
+
+
+def msm_dev_batch(curve, d_points, d_scalars, nbits=None, stream=None):
+    """B scalar vectors against one device point set in one call: torch CUDA tensors, d_points packed
+    affine as for msm_dev, d_scalars (B, n, 4) or (B, n, 2) int64, or (B, n) int64 or int32 (the
+    msm_dev conventions, plain integers, bits from `nbits` up ignored).  Synchronises the stream and
+    returns (B, 3 * limbs) uint64, row b the Jacobian result of vector b."""
+    import torch
+    nl = _LIMBS[curve]
+    assert d_points.is_cuda and d_scalars.is_cuda and d_points.is_contiguous() and d_scalars.is_contiguous()
+    sbytes, B, n = _batch_format(d_scalars, torch.int64, torch.int32)
+    fmt = _scalar_format(sbytes, False, nbits) or (32, 255)
+    out = np.zeros((B, 3 * nl), dtype=np.uint64)
+    with torch.cuda.device(d_points.device):
+        s = stream if stream is not None else torch.cuda.current_stream().cuda_stream
+        err = _lib.lib().sppark_b200_msm_dev_batch(curve, out.ctypes.data, d_points.data_ptr(), n,
+                                                   d_scalars.data_ptr(), B, fmt[0], fmt[1], s)
     _lib.check(err)
     return out
 
