@@ -1,7 +1,5 @@
 // NTT instantiations and their C-ABI entry points (include/sppark_b200.h).
-#include "../ff/gl64.cuh"
-#include "../ff/bb31.cuh"
-#include "../ff/mont_ntt.cuh"
+#include "../ff/field_dispatch.cuh"
 #include "ntt.cuh"
 #include <memory>
 #include <vector>
@@ -26,14 +24,9 @@ static bool try_static(const Pass& d, const Tables<F>& tb, const typename F::T* 
         (d.in_rev != 0) != IREV || (d.out_rev != 0) != OREV || d.tw_mode != TW)
         return false;
     typedef KStat<R, W, IRF, ORF, IREV, OREV, TW> K;
-    // function attributes are per device (context): one flag per CUDA device and instantiation
     int dev = 0;
     CUDA_OK(cudaGetDevice(&dev));
-    static bool attr_done[64];
-    if (!attr_done[dev & 63]) {
-        CUDA_OK(cudaFuncSetAttribute(pass_kernel_static<F, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));   // + the static mbarrier word <= 227 KiB
-        attr_done[dev & 63] = true;
-    }
+    smem_opt_in<pass_kernel_static<F, K>>(dev, 226 * 1024);      // + the static mbarrier word <= 227 KiB
     // one CTA per SM (a tile fills the shared memory), each walking ntiles / grid tiles
     static int sms_of[64];
     if (!sms_of[dev & 63]) CUDA_OK(cudaDeviceGetAttribute(&sms_of[dev & 63], cudaDevAttrMultiProcessorCount, dev));
@@ -127,93 +120,21 @@ template class NTT<ff::bn254_fr_ntt>;
 template class NTT<ff::bls12_377_fr_ntt>;
 }  // namespace ntt
 
+// order 0..4 (NN, NR, RN, RR, BB), direction 0..1, type 0..1: anything else is refused, with the
+// entry's own message, before any work
+static bool bad_ntt_args(int order, int direction, int type)
+{   return order < 0 || order > 4 || direction < 0 || direction > 1 || type < 0 || type > 1;   }
+
 template<class F>
 static RustError ntt_host(size_t device_id, void* inout, uint32_t lg, int order, int direction, int type)
 {
     typedef ntt::NTT<F> N;
-    if (order < 0 || order > 4 || direction < 0 || direction > 1 || type < 0 || type > 1)
+    if (bad_ntt_args(order, direction, type))
         return rust_err(-(int)cudaErrorInvalidValue, "compute_ntt: bad order/direction/type");
-    try {
-        const gpu_t& gpu = select_gpu((int)device_id);
-        return N::Base(gpu, (typename F::T*)inout, lg, (typename N::InputOutputOrder)order,
+    return guarded([&] {
+        return N::Base(select_gpu((int)device_id), (typename F::T*)inout, lg, (typename N::InputOutputOrder)order,
                        (typename N::Direction)direction, (typename N::Type)type);
-    } catch (const cuda_error& e) {
-        return rust_err(e.code(), e.what());
-    } catch (const std::exception& e) {
-        return rust_err(-1, e.what());
-    }
-}
-
-template<class F>
-static RustError ntt_dev(void* d_inout, uint32_t lg, int order, int direction, int type, void* stream)
-{
-    typedef ntt::NTT<F> N;
-    if (order < 0 || order > 4 || direction < 0 || direction > 1 || type < 0 || type > 1)
-        return rust_err(-(int)cudaErrorInvalidValue, "ntt_dev: bad order/direction/type");
-    try {
-        const gpu_t& gpu = gpu_of_current_device();
-        N::Base_dev_ptr(gpu, (cudaStream_t)stream, (typename F::T*)d_inout, lg,
-                        (typename N::InputOutputOrder)order, (typename N::Direction)direction,
-                        (typename N::Type)type);
-        return rust_ok();
-    } catch (const cuda_error& e) {
-        return rust_err(e.code(), e.what());
-    } catch (const std::exception& e) {
-        return rust_err(-1, e.what());
-    }
-}
-
-template<class F>
-static RustError ntt_batch_host(size_t device_id, void* inout, uint32_t lg, size_t batch, int order, int direction,
-                                int type)
-{
-    typedef ntt::NTT<F> N;
-    if (order < 0 || order > 4 || direction < 0 || direction > 1 || type < 0 || type > 1)
-        return rust_err(-(int)cudaErrorInvalidValue, "ntt_batch: bad order/direction/type");
-    try {
-        const gpu_t& gpu = select_gpu((int)device_id);
-        return N::Base_batch(gpu, (typename F::T*)inout, lg, batch, (typename N::InputOutputOrder)order,
-                             (typename N::Direction)direction, (typename N::Type)type);
-    } catch (const cuda_error& e) {
-        return rust_err(e.code(), e.what());
-    } catch (const std::exception& e) {
-        return rust_err(-1, e.what());
-    }
-}
-
-template<class F>
-static RustError ntt_batch_dev(void* d_inout, uint32_t lg, size_t batch, int order, int direction, int type,
-                               void* stream)
-{
-    typedef ntt::NTT<F> N;
-    if (order < 0 || order > 4 || direction < 0 || direction > 1 || type < 0 || type > 1)
-        return rust_err(-(int)cudaErrorInvalidValue, "ntt_batch_dev: bad order/direction/type");
-    if (lg > (uint32_t)F::MAX_LG || !N::batch_fits(lg, batch))
-        return rust_err(-(int)cudaErrorInvalidValue, "ntt_batch_dev: lg_domain_size or batch out of range for this field");
-    try {
-        const gpu_t& gpu = gpu_of_current_device();
-        N::NTT_internal(gpu, (typename F::T*)d_inout, lg, (typename N::InputOutputOrder)order,
-                        (typename N::Direction)direction, (typename N::Type)type, (cudaStream_t)stream, batch);
-        return rust_ok();
-    } catch (const cuda_error& e) {
-        return rust_err(e.code(), e.what());
-    } catch (const std::exception& e) {
-        return rust_err(-1, e.what());
-    }
-}
-
-template<class F>
-static RustError lde_batch_dev(void* d_out, void* d_in, uint32_t lg, uint32_t lg_blowup, size_t batch, void* stream)
-{
-    try {
-        ntt::NTT<F>::LDE_batch_dev(gpu_of_current_device(), (cudaStream_t)stream, (typename F::T*)d_out,
-                                   (typename F::T*)d_in, lg, lg_blowup, batch);
-        return rust_ok();
-    } catch (const cuda_error& e) {
-        return rust_err(e.code(), e.what());
-    } catch (const std::exception& e) {
-        return rust_err(-1, e.what());
-    }
+    });
 }
 
 template<class F>
@@ -223,105 +144,63 @@ static RustError ntt_slab(int which, const void* d_in, void* d_out, uint32_t lg,
     typedef ntt::NTT<F> N;
     if (direction < 0 || direction > 1 || (which != 1 && which != 2))
         return rust_err(-(int)cudaErrorInvalidValue, "ntt_slab_pass: bad direction / pass");
-    try {
+    return guarded([&] {
         N::slab_pass(gpu_of_current_device(), which, (const typename F::T*)d_in, (typename F::T*)d_out, lg, lg_g,
                      rank, (typename N::Direction)direction, (cudaStream_t)stream, peers);
         return rust_ok();
-    } catch (const cuda_error& e) {
-        return rust_err(e.code(), e.what());
-    } catch (const std::exception& e) {
-        return rust_err(-1, e.what());
-    }
+    });
 }
 
-template<class F>
-static RustError lde_host(size_t device_id, void* inout, uint32_t lg, uint32_t lg_blowup, void* aux)
-{
-    try {
-        return ntt::NTT<F>::LDE(select_gpu((int)device_id), (typename F::T*)inout, lg, lg_blowup, (typename F::T*)aux);
-    } catch (const cuda_error& e) {
-        return rust_err(e.code(), e.what());
-    } catch (const std::exception& e) {
-        return rust_err(-1, e.what());
-    }
-}
-
-template<class F>
-static RustError lde_dev(int what, void* d_out, const void* d_in, uint32_t lg, uint32_t lg_blowup, void* stream)
-{
-    try {
-        const gpu_t& gpu = gpu_of_current_device();
-        if (what == 0) ntt::NTT<F>::LDE_powers(gpu, (cudaStream_t)stream, (typename F::T*)d_out, lg);
-        else ntt::NTT<F>::LDE_expand(gpu, (cudaStream_t)stream, (typename F::T*)d_out, (const typename F::T*)d_in, lg, lg_blowup);
-        return rust_ok();
-    } catch (const cuda_error& e) {
-        return rust_err(e.code(), e.what());
-    } catch (const std::exception& e) {
-        return rust_err(-1, e.what());
-    }
-}
-static RustError lde_dev_any(int field, int what, void* d_out, const void* d_in, uint32_t lg, uint32_t lb, void* stream)
-{
-    switch (field) {
-    case SPPARK_FIELD_GL64: return lde_dev<gl64>(what, d_out, d_in, lg, lb, stream);
-    case SPPARK_FIELD_BB31: return lde_dev<bb31>(what, d_out, d_in, lg, lb, stream);
-    case SPPARK_FIELD_BLS12_381_FR: return lde_dev<ff::bls12_381_fr_ntt>(what, d_out, d_in, lg, lb, stream);
-    case SPPARK_FIELD_PALLAS_FR: return lde_dev<ff::pallas_fr_ntt>(what, d_out, d_in, lg, lb, stream);
-    case SPPARK_FIELD_VESTA_FR: return lde_dev<ff::vesta_fr_ntt>(what, d_out, d_in, lg, lb, stream);
-    case SPPARK_FIELD_BN254_FR: return lde_dev<ff::bn254_fr_ntt>(what, d_out, d_in, lg, lb, stream);
-    case SPPARK_FIELD_BLS12_377_FR: return lde_dev<ff::bls12_377_fr_ntt>(what, d_out, d_in, lg, lb, stream);
-    default: return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_lde_*_dev: unknown field");
-    }
-}
 extern "C" RustError sppark_b200_lde_powers_dev(int field, void* d_inout, uint32_t lg, void* stream)
-{   return lde_dev_any(field, 0, d_inout, nullptr, lg, 0, stream);   }
+{
+    return with_field(field, "sppark_b200_lde_*_dev: unknown field", [&](auto t) {
+        typedef typename decltype(t)::type F;
+        return guarded([&] {
+            ntt::NTT<F>::LDE_powers(gpu_of_current_device(), (cudaStream_t)stream, (typename F::T*)d_inout, lg);
+            return rust_ok();
+        });
+    });
+}
+
 extern "C" RustError sppark_b200_lde_expand_dev(int field, void* d_out, const void* d_in, uint32_t lg,
                                                 uint32_t lg_blowup, void* stream)
-{   return lde_dev_any(field, 1, d_out, d_in, lg, lg_blowup, stream);   }
+{
+    return with_field(field, "sppark_b200_lde_*_dev: unknown field", [&](auto t) {
+        typedef typename decltype(t)::type F;
+        return guarded([&] {
+            ntt::NTT<F>::LDE_expand(gpu_of_current_device(), (cudaStream_t)stream, (typename F::T*)d_out,
+                                    (const typename F::T*)d_in, lg, lg_blowup);
+            return rust_ok();
+        });
+    });
+}
 
 extern "C" RustError sppark_b200_lde(int field, size_t device_id, void* inout, uint32_t lg, uint32_t lg_blowup, void* aux_out)
 {
-    switch (field) {
-    case SPPARK_FIELD_GL64: return lde_host<gl64>(device_id, inout, lg, lg_blowup, aux_out);
-    case SPPARK_FIELD_BB31: return lde_host<bb31>(device_id, inout, lg, lg_blowup, aux_out);
-    case SPPARK_FIELD_BLS12_381_FR: return lde_host<ff::bls12_381_fr_ntt>(device_id, inout, lg, lg_blowup, aux_out);
-    case SPPARK_FIELD_PALLAS_FR: return lde_host<ff::pallas_fr_ntt>(device_id, inout, lg, lg_blowup, aux_out);
-    case SPPARK_FIELD_VESTA_FR: return lde_host<ff::vesta_fr_ntt>(device_id, inout, lg, lg_blowup, aux_out);
-    case SPPARK_FIELD_BN254_FR: return lde_host<ff::bn254_fr_ntt>(device_id, inout, lg, lg_blowup, aux_out);
-    case SPPARK_FIELD_BLS12_377_FR: return lde_host<ff::bls12_377_fr_ntt>(device_id, inout, lg, lg_blowup, aux_out);
-    default: return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_lde: unknown field");
-    }
+    return with_field(field, "sppark_b200_lde: unknown field", [&](auto t) {
+        typedef typename decltype(t)::type F;
+        return guarded([&] {
+            return ntt::NTT<F>::LDE(select_gpu((int)device_id), (typename F::T*)inout, lg, lg_blowup,
+                                    (typename F::T*)aux_out);
+        });
+    });
 }
 
 extern "C" RustError sppark_b200_ntt_slab_pass(int field, int which, const void* d_in, void* d_out,
                                                uint32_t lg, uint32_t lg_g, uint32_t rank, int direction, void* stream)
 {
-    switch (field) {
-    case SPPARK_FIELD_GL64: return ntt_slab<gl64>(which, d_in, d_out, lg, lg_g, rank, direction, stream);
-    case SPPARK_FIELD_BB31: return ntt_slab<bb31>(which, d_in, d_out, lg, lg_g, rank, direction, stream);
-    case SPPARK_FIELD_BLS12_381_FR: return ntt_slab<ff::bls12_381_fr_ntt>(which, d_in, d_out, lg, lg_g, rank, direction, stream);
-    case SPPARK_FIELD_PALLAS_FR: return ntt_slab<ff::pallas_fr_ntt>(which, d_in, d_out, lg, lg_g, rank, direction, stream);
-    case SPPARK_FIELD_VESTA_FR: return ntt_slab<ff::vesta_fr_ntt>(which, d_in, d_out, lg, lg_g, rank, direction, stream);
-    case SPPARK_FIELD_BN254_FR: return ntt_slab<ff::bn254_fr_ntt>(which, d_in, d_out, lg, lg_g, rank, direction, stream);
-    case SPPARK_FIELD_BLS12_377_FR: return ntt_slab<ff::bls12_377_fr_ntt>(which, d_in, d_out, lg, lg_g, rank, direction, stream);
-    default: return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_ntt_slab_pass: unknown field");
-    }
+    return with_field(field, "sppark_b200_ntt_slab_pass: unknown field", [&](auto t) {
+        return ntt_slab<typename decltype(t)::type>(which, d_in, d_out, lg, lg_g, rank, direction, stream);
+    });
 }
 
 extern "C" RustError sppark_b200_ntt_slab_pass_p2p(int field, const void* d_in, void* const* peer_recv,
                                                    uint32_t lg, uint32_t lg_g, uint32_t rank, int direction, void* stream)
 {
     if (peer_recv == nullptr) return rust_err(-(int)cudaErrorInvalidValue, "ntt_slab_pass_p2p: no peer buffers");
-    switch (field) {
-    case SPPARK_FIELD_GL64: return ntt_slab<gl64>(1, d_in, nullptr, lg, lg_g, rank, direction, stream, peer_recv);
-    case SPPARK_FIELD_BB31: return ntt_slab<bb31>(1, d_in, nullptr, lg, lg_g, rank, direction, stream, peer_recv);
-    case SPPARK_FIELD_BLS12_381_FR: return ntt_slab<ff::bls12_381_fr_ntt>(1, d_in, nullptr, lg, lg_g, rank, direction, stream, peer_recv);
-    case SPPARK_FIELD_PALLAS_FR: return ntt_slab<ff::pallas_fr_ntt>(1, d_in, nullptr, lg, lg_g, rank, direction, stream, peer_recv);
-    case SPPARK_FIELD_VESTA_FR: return ntt_slab<ff::vesta_fr_ntt>(1, d_in, nullptr, lg, lg_g, rank, direction, stream, peer_recv);
-    case SPPARK_FIELD_BN254_FR: return ntt_slab<ff::bn254_fr_ntt>(1, d_in, nullptr, lg, lg_g, rank, direction, stream, peer_recv);
-    case SPPARK_FIELD_BLS12_377_FR: return ntt_slab<ff::bls12_377_fr_ntt>(1, d_in, nullptr, lg, lg_g, rank, direction, stream, peer_recv);
-    default: return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_ntt_slab_pass_p2p: unknown field");
-    }
+    return with_field(field, "sppark_b200_ntt_slab_pass_p2p: unknown field", [&](auto t) {
+        return ntt_slab<typename decltype(t)::type>(1, d_in, nullptr, lg, lg_g, rank, direction, stream, peer_recv);
+    });
 }
 
 // ---- one transform slab-sharded over several GPUs of THIS process (SURVEY.md section 8e) -----------
@@ -453,16 +332,9 @@ extern "C" RustError sppark_b200_ntt_sharded(int field, void* inout, uint32_t lg
     for (size_t i = 0; i < ndev; i++)
         if (device_ids[i] < 0 || device_ids[i] >= count)
             return rust_err(-(int)cudaErrorInvalidDevice, "ntt_sharded: no such device");
-    switch (field) {
-    case SPPARK_FIELD_GL64: return ntt_sharded<gl64>(inout, lg_domain_size, ntt_direction, device_ids, ndev);
-    case SPPARK_FIELD_BB31: return ntt_sharded<bb31>(inout, lg_domain_size, ntt_direction, device_ids, ndev);
-    case SPPARK_FIELD_BLS12_381_FR: return ntt_sharded<ff::bls12_381_fr_ntt>(inout, lg_domain_size, ntt_direction, device_ids, ndev);
-    case SPPARK_FIELD_PALLAS_FR: return ntt_sharded<ff::pallas_fr_ntt>(inout, lg_domain_size, ntt_direction, device_ids, ndev);
-    case SPPARK_FIELD_VESTA_FR: return ntt_sharded<ff::vesta_fr_ntt>(inout, lg_domain_size, ntt_direction, device_ids, ndev);
-    case SPPARK_FIELD_BN254_FR: return ntt_sharded<ff::bn254_fr_ntt>(inout, lg_domain_size, ntt_direction, device_ids, ndev);
-    case SPPARK_FIELD_BLS12_377_FR: return ntt_sharded<ff::bls12_377_fr_ntt>(inout, lg_domain_size, ntt_direction, device_ids, ndev);
-    default: return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_ntt_sharded: unknown field");
-    }
+    return with_field(field, "sppark_b200_ntt_sharded: unknown field", [&](auto t) {
+        return ntt_sharded<typename decltype(t)::type>(inout, lg_domain_size, ntt_direction, device_ids, ndev);
+    });
 }
 
 extern "C" RustError compute_ntt(size_t device_id, void* inout, uint32_t lg_domain_size,
@@ -472,174 +344,127 @@ extern "C" RustError compute_ntt(size_t device_id, void* inout, uint32_t lg_doma
 extern "C" RustError sppark_b200_ntt(int field, size_t device_id, void* inout, uint32_t lg,
                                      int order, int direction, int type)
 {
-    switch (field) {
-    case SPPARK_FIELD_GL64: return ntt_host<gl64>(device_id, inout, lg, order, direction, type);
-    case SPPARK_FIELD_BB31: return ntt_host<bb31>(device_id, inout, lg, order, direction, type);
-    case SPPARK_FIELD_BLS12_381_FR: return ntt_host<ff::bls12_381_fr_ntt>(device_id, inout, lg, order, direction, type);
-    case SPPARK_FIELD_PALLAS_FR: return ntt_host<ff::pallas_fr_ntt>(device_id, inout, lg, order, direction, type);
-    case SPPARK_FIELD_VESTA_FR: return ntt_host<ff::vesta_fr_ntt>(device_id, inout, lg, order, direction, type);
-    case SPPARK_FIELD_BN254_FR: return ntt_host<ff::bn254_fr_ntt>(device_id, inout, lg, order, direction, type);
-    case SPPARK_FIELD_BLS12_377_FR: return ntt_host<ff::bls12_377_fr_ntt>(device_id, inout, lg, order, direction, type);
-    default: return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_ntt: unknown field");
-    }
+    return with_field(field, "sppark_b200_ntt: unknown field", [&](auto t) {
+        return ntt_host<typename decltype(t)::type>(device_id, inout, lg, order, direction, type);
+    });
 }
 
 extern "C" RustError sppark_b200_ntt_dev(int field, void* d_inout, uint32_t lg, int order,
                                          int direction, int type, void* stream)
 {
-    switch (field) {
-    case SPPARK_FIELD_GL64: return ntt_dev<gl64>(d_inout, lg, order, direction, type, stream);
-    case SPPARK_FIELD_BB31: return ntt_dev<bb31>(d_inout, lg, order, direction, type, stream);
-    case SPPARK_FIELD_BLS12_381_FR: return ntt_dev<ff::bls12_381_fr_ntt>(d_inout, lg, order, direction, type, stream);
-    case SPPARK_FIELD_PALLAS_FR: return ntt_dev<ff::pallas_fr_ntt>(d_inout, lg, order, direction, type, stream);
-    case SPPARK_FIELD_VESTA_FR: return ntt_dev<ff::vesta_fr_ntt>(d_inout, lg, order, direction, type, stream);
-    case SPPARK_FIELD_BN254_FR: return ntt_dev<ff::bn254_fr_ntt>(d_inout, lg, order, direction, type, stream);
-    case SPPARK_FIELD_BLS12_377_FR: return ntt_dev<ff::bls12_377_fr_ntt>(d_inout, lg, order, direction, type, stream);
-    default: return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_ntt_dev: unknown field");
-    }
+    return with_field(field, "sppark_b200_ntt_dev: unknown field", [&](auto t) {
+        typedef typename decltype(t)::type F;
+        typedef ntt::NTT<F> N;
+        if (bad_ntt_args(order, direction, type))
+            return rust_err(-(int)cudaErrorInvalidValue, "ntt_dev: bad order/direction/type");
+        return guarded([&] {
+            N::Base_dev_ptr(gpu_of_current_device(), (cudaStream_t)stream, (typename F::T*)d_inout, lg,
+                            (typename N::InputOutputOrder)order, (typename N::Direction)direction,
+                            (typename N::Type)type);
+            return rust_ok();
+        });
+    });
 }
 
 extern "C" RustError sppark_b200_ntt_batch_dev(int field, void* d_inout, uint32_t lg, size_t batch, int order,
                                                int direction, int type, void* stream)
 {
-    switch (field) {
-    case SPPARK_FIELD_GL64: return ntt_batch_dev<gl64>(d_inout, lg, batch, order, direction, type, stream);
-    case SPPARK_FIELD_BB31: return ntt_batch_dev<bb31>(d_inout, lg, batch, order, direction, type, stream);
-    case SPPARK_FIELD_BLS12_381_FR: return ntt_batch_dev<ff::bls12_381_fr_ntt>(d_inout, lg, batch, order, direction, type, stream);
-    case SPPARK_FIELD_PALLAS_FR: return ntt_batch_dev<ff::pallas_fr_ntt>(d_inout, lg, batch, order, direction, type, stream);
-    case SPPARK_FIELD_VESTA_FR: return ntt_batch_dev<ff::vesta_fr_ntt>(d_inout, lg, batch, order, direction, type, stream);
-    case SPPARK_FIELD_BN254_FR: return ntt_batch_dev<ff::bn254_fr_ntt>(d_inout, lg, batch, order, direction, type, stream);
-    case SPPARK_FIELD_BLS12_377_FR: return ntt_batch_dev<ff::bls12_377_fr_ntt>(d_inout, lg, batch, order, direction, type, stream);
-    default: return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_ntt_batch_dev: unknown field");
-    }
+    return with_field(field, "sppark_b200_ntt_batch_dev: unknown field", [&](auto t) {
+        typedef typename decltype(t)::type F;
+        typedef ntt::NTT<F> N;
+        if (bad_ntt_args(order, direction, type))
+            return rust_err(-(int)cudaErrorInvalidValue, "ntt_batch_dev: bad order/direction/type");
+        if (lg > (uint32_t)F::MAX_LG || !N::batch_fits(lg, batch))
+            return rust_err(-(int)cudaErrorInvalidValue, "ntt_batch_dev: lg_domain_size or batch out of range for this field");
+        return guarded([&] {
+            N::NTT_internal(gpu_of_current_device(), (typename F::T*)d_inout, lg, (typename N::InputOutputOrder)order,
+                            (typename N::Direction)direction, (typename N::Type)type, (cudaStream_t)stream, batch);
+            return rust_ok();
+        });
+    });
 }
 
 extern "C" RustError sppark_b200_lde_batch_dev(int field, void* d_out, void* d_in, uint32_t lg, uint32_t lg_blowup,
                                                size_t batch, void* stream)
 {
-    switch (field) {
-    case SPPARK_FIELD_GL64: return lde_batch_dev<gl64>(d_out, d_in, lg, lg_blowup, batch, stream);
-    case SPPARK_FIELD_BB31: return lde_batch_dev<bb31>(d_out, d_in, lg, lg_blowup, batch, stream);
-    case SPPARK_FIELD_BLS12_381_FR: return lde_batch_dev<ff::bls12_381_fr_ntt>(d_out, d_in, lg, lg_blowup, batch, stream);
-    case SPPARK_FIELD_PALLAS_FR: return lde_batch_dev<ff::pallas_fr_ntt>(d_out, d_in, lg, lg_blowup, batch, stream);
-    case SPPARK_FIELD_VESTA_FR: return lde_batch_dev<ff::vesta_fr_ntt>(d_out, d_in, lg, lg_blowup, batch, stream);
-    case SPPARK_FIELD_BN254_FR: return lde_batch_dev<ff::bn254_fr_ntt>(d_out, d_in, lg, lg_blowup, batch, stream);
-    case SPPARK_FIELD_BLS12_377_FR: return lde_batch_dev<ff::bls12_377_fr_ntt>(d_out, d_in, lg, lg_blowup, batch, stream);
-    default: return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_lde_batch_dev: unknown field");
-    }
+    return with_field(field, "sppark_b200_lde_batch_dev: unknown field", [&](auto t) {
+        typedef typename decltype(t)::type F;
+        return guarded([&] {
+            ntt::NTT<F>::LDE_batch_dev(gpu_of_current_device(), (cudaStream_t)stream, (typename F::T*)d_out,
+                                       (typename F::T*)d_in, lg, lg_blowup, batch);
+            return rust_ok();
+        });
+    });
 }
 
 extern "C" RustError sppark_b200_ntt_batch(int field, size_t device_id, void* inout, uint32_t lg, size_t batch,
                                            int order, int direction, int type)
 {
-    switch (field) {
-    case SPPARK_FIELD_GL64: return ntt_batch_host<gl64>(device_id, inout, lg, batch, order, direction, type);
-    case SPPARK_FIELD_BB31: return ntt_batch_host<bb31>(device_id, inout, lg, batch, order, direction, type);
-    case SPPARK_FIELD_BLS12_381_FR: return ntt_batch_host<ff::bls12_381_fr_ntt>(device_id, inout, lg, batch, order, direction, type);
-    case SPPARK_FIELD_PALLAS_FR: return ntt_batch_host<ff::pallas_fr_ntt>(device_id, inout, lg, batch, order, direction, type);
-    case SPPARK_FIELD_VESTA_FR: return ntt_batch_host<ff::vesta_fr_ntt>(device_id, inout, lg, batch, order, direction, type);
-    case SPPARK_FIELD_BN254_FR: return ntt_batch_host<ff::bn254_fr_ntt>(device_id, inout, lg, batch, order, direction, type);
-    case SPPARK_FIELD_BLS12_377_FR: return ntt_batch_host<ff::bls12_377_fr_ntt>(device_id, inout, lg, batch, order, direction, type);
-    default: return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_ntt_batch: unknown field");
-    }
+    return with_field(field, "sppark_b200_ntt_batch: unknown field", [&](auto t) {
+        typedef typename decltype(t)::type F;
+        typedef ntt::NTT<F> N;
+        if (bad_ntt_args(order, direction, type))
+            return rust_err(-(int)cudaErrorInvalidValue, "ntt_batch: bad order/direction/type");
+        return guarded([&] {
+            return N::Base_batch(select_gpu((int)device_id), (typename F::T*)inout, lg, batch,
+                                 (typename N::InputOutputOrder)order, (typename N::Direction)direction,
+                                 (typename N::Type)type);
+        });
+    });
 }
 
 // ---- NTT and LDE down the columns of a row-major matrix (ntt.cuh: NTTMatrix), Goldilocks and BabyBear ----
-static bool matrix_bad_args(int order, int direction, int type)
-{   return order < 0 || order > 4 || direction < 0 || direction > 1 || type < 0 || type > 1;   }
-
-template<class F>
-static RustError ntt_matrix_dev(void* d_inout, uint32_t lg, size_t width, int order, int direction, int type,
-                                void* stream)
-{
-    typedef ntt::NTT<F> N;
-    if (matrix_bad_args(order, direction, type))
-        return rust_err(-(int)cudaErrorInvalidValue, "ntt_matrix_dev: bad order/direction/type");
-    if (lg > (uint32_t)F::MAX_LG || !ntt::NTTMatrix<F>::fits(lg, width))
-        return rust_err(-(int)cudaErrorInvalidValue, "ntt_matrix_dev: lg_domain_size or width out of range for this field");
-    try {
-        ntt::NTTMatrix<F>::transform(gpu_of_current_device(), (typename F::T*)d_inout, lg, width,
-                                     (typename N::InputOutputOrder)order, (typename N::Direction)direction,
-                                     (typename N::Type)type, (cudaStream_t)stream);
-        return rust_ok();
-    } catch (const cuda_error& e) {
-        return rust_err(e.code(), e.what());
-    } catch (const std::exception& e) {
-        return rust_err(-1, e.what());
-    }
-}
-
-template<class F>
-static RustError lde_matrix_dev(void* d_out, void* d_in, uint32_t lg, uint32_t lg_blowup, size_t width, void* stream)
-{
-    try {
-        ntt::NTTMatrix<F>::LDE_dev(gpu_of_current_device(), (cudaStream_t)stream, (typename F::T*)d_out,
-                                   (typename F::T*)d_in, lg, lg_blowup, width);
-        return rust_ok();
-    } catch (const cuda_error& e) {
-        return rust_err(e.code(), e.what());
-    } catch (const std::exception& e) {
-        return rust_err(-1, e.what());
-    }
-}
-
-template<class F>
-static RustError ntt_matrix_host(size_t device_id, void* inout, uint32_t lg, size_t width, int order, int direction,
-                                 int type)
-{
-    typedef ntt::NTT<F> N;
-    if (matrix_bad_args(order, direction, type))
-        return rust_err(-(int)cudaErrorInvalidValue, "ntt_matrix: bad order/direction/type");
-    if (lg > (uint32_t)F::MAX_LG || !ntt::NTTMatrix<F>::fits(lg, width))
-        return rust_err(-(int)cudaErrorInvalidValue, "ntt_matrix: lg_domain_size or width out of range for this field");
-    if (lg == 0 || width == 0) return rust_ok();
-    try {
-        return ntt::NTTMatrix<F>::host(select_gpu((int)device_id), (typename F::T*)inout, lg, width,
-                                       (typename N::InputOutputOrder)order, (typename N::Direction)direction,
-                                       (typename N::Type)type);
-    } catch (const cuda_error& e) {
-        return rust_err(e.code(), e.what());
-    } catch (const std::exception& e) {
-        return rust_err(-1, e.what());
-    }
-}
-
-static RustError matrix_field_refused(int field, const char* entry)
-{
-    static const std::string wide = ": the matrix entries serve Goldilocks and BabyBear only, not the 256-bit fields";
-    static const std::string unknown = ": unknown field";
-    const bool is_wide = field == SPPARK_FIELD_BLS12_381_FR || field == SPPARK_FIELD_PALLAS_FR ||
-                         field == SPPARK_FIELD_VESTA_FR || field == SPPARK_FIELD_BN254_FR ||
-                         field == SPPARK_FIELD_BLS12_377_FR;
-    return rust_err(-(int)cudaErrorInvalidValue, (std::string(entry) + (is_wide ? wide : unknown)).c_str());
-}
+// an entry's refusals of an unknown field id and of a 256-bit field's id
+#define MATRIX_REFUSALS(entry) \
+    entry ": unknown field", entry ": the matrix entries serve Goldilocks and BabyBear only, not the 256-bit fields"
 
 extern "C" RustError sppark_b200_ntt_matrix_dev(int field, void* d_inout, uint32_t lg, size_t width, int order,
                                                 int direction, int type, void* stream)
 {
-    switch (field) {
-    case SPPARK_FIELD_GL64: return ntt_matrix_dev<gl64>(d_inout, lg, width, order, direction, type, stream);
-    case SPPARK_FIELD_BB31: return ntt_matrix_dev<bb31>(d_inout, lg, width, order, direction, type, stream);
-    default: return matrix_field_refused(field, "sppark_b200_ntt_matrix_dev");
-    }
+    return with_word_field(field, MATRIX_REFUSALS("sppark_b200_ntt_matrix_dev"), [&](auto t) {
+        typedef typename decltype(t)::type F;
+        typedef ntt::NTT<F> N;
+        if (bad_ntt_args(order, direction, type))
+            return rust_err(-(int)cudaErrorInvalidValue, "ntt_matrix_dev: bad order/direction/type");
+        if (lg > (uint32_t)F::MAX_LG || !ntt::NTTMatrix<F>::fits(lg, width))
+            return rust_err(-(int)cudaErrorInvalidValue, "ntt_matrix_dev: lg_domain_size or width out of range for this field");
+        return guarded([&] {
+            ntt::NTTMatrix<F>::transform(gpu_of_current_device(), (typename F::T*)d_inout, lg, width,
+                                         (typename N::InputOutputOrder)order, (typename N::Direction)direction,
+                                         (typename N::Type)type, (cudaStream_t)stream);
+            return rust_ok();
+        });
+    });
 }
 
 extern "C" RustError sppark_b200_lde_matrix_dev(int field, void* d_out, void* d_in, uint32_t lg, uint32_t lg_blowup,
                                                 size_t width, void* stream)
 {
-    switch (field) {
-    case SPPARK_FIELD_GL64: return lde_matrix_dev<gl64>(d_out, d_in, lg, lg_blowup, width, stream);
-    case SPPARK_FIELD_BB31: return lde_matrix_dev<bb31>(d_out, d_in, lg, lg_blowup, width, stream);
-    default: return matrix_field_refused(field, "sppark_b200_lde_matrix_dev");
-    }
+    return with_word_field(field, MATRIX_REFUSALS("sppark_b200_lde_matrix_dev"), [&](auto t) {
+        typedef typename decltype(t)::type F;
+        return guarded([&] {
+            ntt::NTTMatrix<F>::LDE_dev(gpu_of_current_device(), (cudaStream_t)stream, (typename F::T*)d_out,
+                                       (typename F::T*)d_in, lg, lg_blowup, width);
+            return rust_ok();
+        });
+    });
 }
 
 extern "C" RustError sppark_b200_ntt_matrix(int field, size_t device_id, void* inout, uint32_t lg, size_t width,
                                             int order, int direction, int type)
 {
-    switch (field) {
-    case SPPARK_FIELD_GL64: return ntt_matrix_host<gl64>(device_id, inout, lg, width, order, direction, type);
-    case SPPARK_FIELD_BB31: return ntt_matrix_host<bb31>(device_id, inout, lg, width, order, direction, type);
-    default: return matrix_field_refused(field, "sppark_b200_ntt_matrix");
-    }
+    return with_word_field(field, MATRIX_REFUSALS("sppark_b200_ntt_matrix"), [&](auto t) {
+        typedef typename decltype(t)::type F;
+        typedef ntt::NTT<F> N;
+        if (bad_ntt_args(order, direction, type))
+            return rust_err(-(int)cudaErrorInvalidValue, "ntt_matrix: bad order/direction/type");
+        if (lg > (uint32_t)F::MAX_LG || !ntt::NTTMatrix<F>::fits(lg, width))
+            return rust_err(-(int)cudaErrorInvalidValue, "ntt_matrix: lg_domain_size or width out of range for this field");
+        if (lg == 0 || width == 0) return rust_ok();
+        return guarded([&] {
+            return ntt::NTTMatrix<F>::host(select_gpu((int)device_id), (typename F::T*)inout, lg, width,
+                                           (typename N::InputOutputOrder)order, (typename N::Direction)direction,
+                                           (typename N::Type)type);
+        });
+    });
 }

@@ -123,14 +123,9 @@ void launch_matrix_pass(const Pass& d, const Tables<F>& tb, const typename F::T*
 {
     int dev = 0;
     CUDA_OK(cudaGetDevice(&dev));
-    static bool attr_done[64];
+    smem_opt_in<matrix_pass_kernel<F, K>>(dev, 226 * 1024);      // + the static mbarrier word <= 227 KiB
     static int sms_of[64];
-    if (!attr_done[dev & 63]) {
-        // + the static mbarrier word <= 227 KiB
-        CUDA_OK(cudaFuncSetAttribute(matrix_pass_kernel<F, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-        CUDA_OK(cudaDeviceGetAttribute(&sms_of[dev & 63], cudaDevAttrMultiProcessorCount, dev));
-        attr_done[dev & 63] = true;
-    }
+    if (!sms_of[dev & 63]) CUDA_OK(cudaDeviceGetAttribute(&sms_of[dev & 63], cudaDevAttrMultiProcessorCount, dev));
     const size_t smem = smem_elems(d) * sizeof(typename F::T);
     const uint32_t threads = tile_threads<F>(d);
     const uint64_t ncb = matrix_col_blocks(d, width), ntiles = ncb << (lg_n - d.lg_r);
@@ -389,20 +384,12 @@ public:
         const bool out_rev = order != InputOutputOrder::NN && order != InputOutputOrder::RN;
 
         // single-word fields: warp-autonomous passes of 2^4..2^8-point sub-NTTs (ntt_warp.cuh);
-        // 256-bit fields (and SPPARK_B200_NTT_BLOCK=1): block-tile passes of up to 2^12 points
+        // 256-bit fields (and SPPARK_B200_NTT_BLOCK=1): block-tile passes of up to 2^12 points.  A
+        // warp-path tile holds up to 64 adjacent columns; the block tiles are sized from all the
+        // transforms of a batch together
         const bool warp_path = use_warp_path(lg_n);
-        uint32_t lg_tile = FieldId<F>::lg_tile;
-        if (warp_path) {
-            lg_tile = WARP_MAX_LG_R + 6;                  // up to 64 adjacent columns per tile
-        } else {
-            // 2^14-element tiles fill one SM's shared memory; below 2^22 elements (all transforms of
-            // a batch together) shrink the tile so that there are still >= 256 of them for the 132 SMs
-            uint32_t lg_total = lg_n;
-            while (lg_total < 63 && (batch >> (lg_total - lg_n)) > 1) lg_total++;   // floor(log2(batch << lg_n))
-            if (lg_total < lg_tile + 8) lg_tile = lg_total > 18 ? lg_total - 8 : 10;
-            if (const char* env = getenv("SPPARK_B200_NTT_LG_TILE")) lg_tile = (uint32_t)atoi(env);
-            if (lg_tile > FieldId<F>::lg_tile) lg_tile = FieldId<F>::lg_tile;
-        }
+        const uint32_t lg_tile = warp_path ? WARP_MAX_LG_R + 6
+                                           : block_lg_tile(lg_n, batch, FieldId<F>::lg_tile, getenv("SPPARK_B200_NTT_LG_TILE"));
         Plan plan = make_plan(lg_n, (int)order, inverse, lg_tile, 6, warp_path ? WARP_MAX_LG_R : F::NTT_MAX_LG_R);
         if (batch > 1) {
             if (!set_batch(plan, batch))
@@ -424,12 +411,7 @@ public:
             CUDA_OK(cudaMallocAsync((void**)&scratch, (sizeof(T) * batch) << lg_n, stream));
         T* buf[2] = {d_inout, scratch};
 
-        static bool attr_done[64];
-        if (!attr_done[gpu.cid() & 63]) {
-            CUDA_OK(cudaFuncSetAttribute(pass_kernel<F>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)gpu.props().sharedMemPerBlockOptin));
-            attr_done[gpu.cid() & 63] = true;
-        }
+        smem_opt_in<pass_kernel<F>>(gpu.cid(), (int)gpu.props().sharedMemPerBlockOptin);
         g_profile.reset();
         for (const Pass& d : plan.passes) {
             g_profile.mark("pass", stream);
@@ -476,22 +458,15 @@ public:
         const bool inverse = direction == Direction::inverse;
         if (lg_n > (uint32_t)F::MAX_LG || lg_n > 30 || rank >= (1u << lg_g))
             throw cuda_error(-(int)cudaErrorInvalidValue, "NTT slab: bad lg_domain_size / rank");
-        uint32_t lg_local = lg_n - lg_g, lg_tile = FieldId<F>::lg_tile;
-        if (lg_local < lg_tile + 8) lg_tile = lg_local > 18 ? lg_local - 8 : 10;
-        if (lg_tile > FieldId<F>::lg_tile) lg_tile = FieldId<F>::lg_tile;
+        const uint32_t lg_local = lg_n - lg_g;
         SlabPlan sp;
-        if (!make_slab_plan(sp, lg_n, lg_g, rank, inverse, lg_tile, F::NTT_MAX_LG_R))
+        if (!make_slab_plan(sp, lg_n, lg_g, rank, inverse, block_lg_tile(lg_local, 1, FieldId<F>::lg_tile), F::NTT_MAX_LG_R))
             throw cuda_error(-(int)cudaErrorInvalidValue,
                              "NTT slab: the first digit of lg_domain_size and the rest must both be >= lg_g");
         if (which == 2 && sp.needs_scratch && d_out == d_in)
             throw cuda_error(-(int)cudaErrorInvalidValue, "NTT slab: this size needs a scratch buffer distinct from the data");
         const Tables<F>& tb = tables(gpu, lg_n, inverse, stream);
-        static bool attr_done[64];
-        if (!attr_done[gpu.cid() & 63]) {
-            CUDA_OK(cudaFuncSetAttribute(pass_kernel<F>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)gpu.props().sharedMemPerBlockOptin));
-            attr_done[gpu.cid() & 63] = true;
-        }
+        smem_opt_in<pass_kernel<F>>(gpu.cid(), (int)gpu.props().sharedMemPerBlockOptin);
         g_profile.reset();
         auto run = [&](const Pass& d, const T* src, T* dst) {
             uint32_t ntiles = 1u << (lg_local - d.lg_r - d.lg_w);
@@ -534,24 +509,18 @@ public:
             const size_t n = (size_t)1 << lg_n, n_ext = (size_t)1 << lg_ext;
             dev_ptr_t<T> d_in(n, s), d_ext(n_ext, s);
             s.HtoD(d_in, inout, n * sizeof(T));
-            NTT_internal(gpu, d_in, lg_n, InputOutputOrder::NR, Direction::inverse, Type::standard, s);
+            LDE_batch_dev(gpu, s, d_ext, d_in, lg_n, lg_blowup, 1);
             if (aux_out) {
-                // natural-order coefficients = the bit-reversal of the NR inverse just computed
-                // (the reference: bit_rev(aux_data, domain_data), ntt/ntt.cuh:312-315)
+                // natural-order coefficients = the bit-reversal of the NR inverse transform that
+                // LDE_batch_dev leaves in d_in (the reference: bit_rev(aux_data, domain_data),
+                // ntt/ntt.cuh:312-315)
                 dev_ptr_t<T> d_aux(n, s);
                 uint32_t bl = (uint32_t)std::min<size_t>((n + 255) / 256, (size_t)gpu.sm_count() * 16);
                 bitrev_copy_kernel<F><<<bl, 256, 0, s>>>(d_aux, d_in, lg_n);
                 COUNT_LAUNCH();
                 CUDA_OK(cudaGetLastError());
                 s.DtoH(aux_out, d_aux, n * sizeof(T));
-                s.sync();
             }
-            const CosetTables& ct = coset_tables(gpu, false, s);
-            uint32_t blocks = (uint32_t)std::min<size_t>((n_ext + 255) / 256, (size_t)gpu.sm_count() * 16);
-            lde_spread_kernel<F><<<blocks, 256, 0, s>>>(d_ext, d_in, lg_n, lg_blowup, ct.g0, ct.g1, ct.g2);
-            COUNT_LAUNCH();
-            CUDA_OK(cudaGetLastError());
-            NTT_internal(gpu, d_ext, lg_ext, InputOutputOrder::RN, Direction::forward, Type::standard, s);
             s.DtoH(inout, d_ext, n_ext * sizeof(T));
             s.sync();
         } catch (const cuda_error& e) {
@@ -710,13 +679,22 @@ public:
         if (lg_n == 0) return rust_ok();
         if (lg_n > (uint32_t)F::MAX_LG || lg_n > 30)          // before touching the caller's buffer
             return rust_err(-(int)cudaErrorInvalidValue, "NTT: lg_domain_size out of range for this field");
+        return host_round_trip(gpu, inout, (size_t)1 << lg_n, [&](T* d_inout, const stream_t& s) {
+            NTT_internal(gpu, d_inout, lg_n, order, direction, type, s);
+        });
+    }
+
+private:
+    // n elements of host memory in place, synchronised, on stream 0: upload, transform(d_inout, stream)
+    // on the device, download.  Pageable buffers (what the reference's Rust / Go callers pass) are
+    // staged through pinned memory by worker threads; registered buffers go straight to the copy engine
+    template<class Transform>
+    static RustError host_round_trip(const gpu_t& gpu, T* inout, size_t n, Transform&& transform)
+    {
         try {
             gpu.select();
             const stream_t& s = gpu[0];
-            size_t n = (size_t)1 << lg_n;
             dev_ptr_t<T> d_inout(n, s);
-            // pageable buffers (what the reference's Rust / Go callers pass) are staged through
-            // pinned memory by worker threads; registered buffers go straight to the copy engine
             const bool pageable = n * sizeof(T) >= ((size_t)8 << 20) && stager_t::is_pageable(inout);
             std::unique_lock<std::mutex> stage_lock(gpu.stage_mtx, std::defer_lock);
             if (pageable) {
@@ -725,7 +703,7 @@ public:
             } else {
                 s.HtoD(d_inout, inout, n * sizeof(T));
             }
-            NTT_internal(gpu, d_inout, lg_n, order, direction, type, s);
+            transform(d_inout.get(), s);
             if (pageable) gpu.stager().DtoH(s, inout, d_inout, n * sizeof(T));
             else s.DtoH(inout, d_inout, n * sizeof(T));
             s.sync();
@@ -760,12 +738,7 @@ struct NTTMatrix {
     // elements in all the tile shrinks so that there are still >= 256 of them for the 132 SMs, as
     // for the batched passes.  DESIGN.md section 4.6 has the measurements.
     static uint32_t lg_tile(uint32_t lg_n, size_t width)
-    {
-        uint32_t lg_total = lg_n, lg_tile = FieldId<F>::lg_tile;
-        while (lg_total < 63 && (width >> (lg_total - lg_n)) > 1) lg_total++;   // floor(log2(width << lg_n))
-        if (lg_total < lg_tile + 8) lg_tile = lg_total > 18 ? lg_total - 8 : 10;
-        return lg_tile > FieldId<F>::lg_tile ? FieldId<F>::lg_tile : lg_tile;
-    }
+    {   return block_lg_tile(lg_n, width, FieldId<F>::lg_tile);   }
 
     static void coset_scale(const gpu_t& gpu, T* d, uint32_t lg_n, size_t width, bool bitrev, bool inverse,
                             cudaStream_t stream)
@@ -855,28 +828,9 @@ struct NTTMatrix {
         if (lg_n > (uint32_t)F::MAX_LG || !fits(lg_n, width))       // before touching the caller's buffer
             return rust_err(-(int)cudaErrorInvalidValue, "NTT matrix: lg_domain_size or width out of range for this field");
         if (lg_n == 0 || width == 0) return rust_ok();
-        try {
-            gpu.select();
-            const stream_t& s = gpu[0];
-            const size_t n = width << lg_n;
-            dev_ptr_t<T> d_inout(n, s);
-            const bool pageable = n * sizeof(T) >= ((size_t)8 << 20) && stager_t::is_pageable(inout);
-            std::unique_lock<std::mutex> stage_lock(gpu.stage_mtx, std::defer_lock);
-            if (pageable) {
-                stage_lock.lock();
-                gpu.stager().HtoD(s, d_inout, inout, n * sizeof(T));
-            } else {
-                s.HtoD(d_inout, inout, n * sizeof(T));
-            }
+        return N::host_round_trip(gpu, inout, width << lg_n, [&](T* d_inout, const stream_t& s) {
             transform(gpu, d_inout, lg_n, width, order, direction, type, s);
-            if (pageable) gpu.stager().DtoH(s, inout, d_inout, n * sizeof(T));
-            else s.DtoH(inout, d_inout, n * sizeof(T));
-            s.sync();
-        } catch (const cuda_error& e) {
-            try { gpu.sync(); } catch (...) {}
-            return rust_err(e.code(), e.what());
-        }
-        return rust_ok();
+        });
     }
 };
 

@@ -51,6 +51,19 @@ inline std::vector<uint32_t> split_digits(uint32_t lg_n, uint32_t max_lg_r = LG_
     return s;
 }
 
+// lg_tile of the block-tile passes over `count` transforms of 2^lg_n elements side by side:
+// max_lg_tile (a tile that fills one SM's shared memory), shrunk below 2^(max_lg_tile + 8) elements
+// in all so that there are still >= 256 tiles for the 132 SMs.  `knob` (the value of an environment
+// variable, experiments and tests) replaces the shrunk value; the result is at most max_lg_tile
+inline uint32_t block_lg_tile(uint32_t lg_n, uint64_t count, uint32_t max_lg_tile, const char* knob = nullptr)
+{
+    uint32_t lg_total = lg_n, lg_tile = max_lg_tile;
+    while (lg_total < 63 && (count >> (lg_total - lg_n)) > 1) lg_total++;   // floor(log2(count << lg_n))
+    if (lg_total < lg_tile + 8) lg_tile = lg_total > 18 ? lg_total - 8 : 10;
+    if (knob) lg_tile = (uint32_t)atoi(knob);
+    return lg_tile > max_lg_tile ? max_lg_tile : lg_tile;
+}
+
 inline Plan make_plan(uint32_t lg_n, int order, bool inverse, uint32_t lg_tile,
                       uint32_t max_lg_w = 6, uint32_t max_lg_r = LG_DENSE)
 {

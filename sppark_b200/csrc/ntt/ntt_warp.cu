@@ -1,7 +1,5 @@
 // Warp-autonomous NTT passes (ntt_warp.cuh) for the single-word fields: instantiations and launcher.
-#include "../ff/gl64.cuh"
-#include "../ff/bb31.cuh"
-#include "../util/gpu.cuh"
+#include "../ff/field_dispatch.cuh"
 #include "ntt_plan.hpp"
 #include "ntt_warp.cuh"
 
@@ -102,34 +100,25 @@ __global__ void word_selftest_kernel(int op, size_t n, typename F::T* r, const t
     r[i] = z;
 }
 
-template<class F>
-static RustError word_selftest(int op, size_t n, void* r, const void* a, const void* b)
-{
-    typedef typename F::T T;
-    try {
-        const gpu_t& gpu = select_gpu(-1);
-        const stream_t& s = gpu[0];
-        dev_ptr_t<T> da(n, s), db(n, s), dr(n, s);
-        s.HtoD(da, a, n * sizeof(T));
-        s.HtoD(db, b, n * sizeof(T));
-        word_selftest_kernel<F><<<(unsigned)((n + 127) / 128), 128, 0, s>>>(op, n, dr, da, db);
-        COUNT_LAUNCH();
-        CUDA_OK(cudaGetLastError());
-        s.DtoH(r, dr, n * sizeof(T));
-        s.sync();
-    } catch (const cuda_error& e) {
-        return rust_err(e.code(), e.what());
-    }
-    return rust_ok();
-}
-
 }  // namespace ntt
 
 extern "C" RustError sppark_b200_selftest_word_field(int field, int op, size_t n, void* r, const void* a, const void* b)
 {
-    switch (field) {
-    case SPPARK_FIELD_GL64: return ntt::word_selftest<gl64>(op, n, r, a, b);
-    case SPPARK_FIELD_BB31: return ntt::word_selftest<bb31>(op, n, r, a, b);
-    default: return rust_err(-(int)cudaErrorInvalidValue, "selftest_word_field: unknown field");
-    }
+    return with_word_field(field, "selftest_word_field: unknown field", nullptr, [&](auto t) {
+        typedef typename decltype(t)::type F;
+        typedef typename F::T T;
+        return guarded([&] {
+            const gpu_t& gpu = select_gpu(-1);
+            const stream_t& s = gpu[0];
+            dev_ptr_t<T> da(n, s), db(n, s), dr(n, s);
+            s.HtoD(da, a, n * sizeof(T));
+            s.HtoD(db, b, n * sizeof(T));
+            ntt::word_selftest_kernel<F><<<(unsigned)((n + 127) / 128), 128, 0, s>>>(op, n, dr, da, db);
+            COUNT_LAUNCH();
+            CUDA_OK(cudaGetLastError());
+            s.DtoH(r, dr, n * sizeof(T));
+            s.sync();
+            return rust_ok();
+        });
+    });
 }

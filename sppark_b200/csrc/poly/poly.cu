@@ -2,6 +2,7 @@
 // Device pointers in, work enqueued on the caller's stream -- the calling convention of the
 // reference's templates (polynomial/prefix_op.cuh:322, div_by_x_minus_z.cuh:445, evaluate.cuh:308),
 // which take device arrays and a stream_t.
+#include "../ff/field_dispatch.cuh"
 #include "poly.cuh"
 
 using namespace poly;
@@ -178,61 +179,46 @@ static void batch_inverse(const gpu_t& gpu, cudaStream_t stream, typename F::T* 
 
 enum { WHAT_PREFIX_ADD, WHAT_PREFIX_MUL, WHAT_DIV, WHAT_EVAL, WHAT_INV };
 
-template<class F>
-static RustError run(int what, void* a, const void* b, size_t n, const void* c, size_t len, int flag, void* stream)
+// every polynomial entry: the field's helper `what` on the caller's stream
+static RustError run(int field, int what, void* a, const void* b, size_t n, const void* c, size_t len, int flag,
+                     void* stream)
 {
-    typedef typename F::T T;
-    try {
-        const gpu_t& gpu = gpu_of_current_device();
-        cudaStream_t s = (cudaStream_t)stream;
-        switch (what) {
-        case WHAT_PREFIX_ADD: scan<F, OP_ADD>(gpu, s, (T*)a, (const T*)b, len, nullptr, 0); break;
-        case WHAT_PREFIX_MUL: scan<F, OP_MUL>(gpu, s, (T*)a, (const T*)b, len, nullptr, 0); break;
-        case WHAT_DIV: scan<F, OP_DIV>(gpu, s, (T*)a, (const T*)a, len, (const T*)c, flag); break;
-        case WHAT_EVAL: evaluate<F>(gpu, s, (T*)a, (const T*)b, n, (const T*)c, len); break;
-        default: batch_inverse<F>(gpu, s, (T*)a, (const T*)b, len); break;
-        }
-        return rust_ok();
-    } catch (const cuda_error& e) {
-        return rust_err(e.code(), e.what());
-    } catch (const std::exception& e) {
-        return rust_err(-1, e.what());
-    }
-}
-
-static RustError run_any(int field, int what, void* a, const void* b, size_t n, const void* c, size_t len, int flag,
-                         void* stream)
-{
-    switch (field) {
-    case SPPARK_FIELD_GL64: return run<gl64>(what, a, b, n, c, len, flag, stream);
-    case SPPARK_FIELD_BB31: return run<bb31>(what, a, b, n, c, len, flag, stream);
-    case SPPARK_FIELD_BLS12_381_FR: return run<ff::bls12_381_fr_ntt>(what, a, b, n, c, len, flag, stream);
-    case SPPARK_FIELD_PALLAS_FR: return run<ff::pallas_fr_ntt>(what, a, b, n, c, len, flag, stream);
-    case SPPARK_FIELD_VESTA_FR: return run<ff::vesta_fr_ntt>(what, a, b, n, c, len, flag, stream);
-    case SPPARK_FIELD_BN254_FR: return run<ff::bn254_fr_ntt>(what, a, b, n, c, len, flag, stream);
-    case SPPARK_FIELD_BLS12_377_FR: return run<ff::bls12_377_fr_ntt>(what, a, b, n, c, len, flag, stream);
-    default: return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200 polynomial: unknown field");
-    }
+    return with_field(field, "sppark_b200 polynomial: unknown field", [&](auto t) {
+        typedef typename decltype(t)::type F;
+        typedef typename F::T T;
+        return guarded([&] {
+            const gpu_t& gpu = gpu_of_current_device();
+            cudaStream_t s = (cudaStream_t)stream;
+            switch (what) {
+            case WHAT_PREFIX_ADD: scan<F, OP_ADD>(gpu, s, (T*)a, (const T*)b, len, nullptr, 0); break;
+            case WHAT_PREFIX_MUL: scan<F, OP_MUL>(gpu, s, (T*)a, (const T*)b, len, nullptr, 0); break;
+            case WHAT_DIV: scan<F, OP_DIV>(gpu, s, (T*)a, (const T*)a, len, (const T*)c, flag); break;
+            case WHAT_EVAL: evaluate<F>(gpu, s, (T*)a, (const T*)b, n, (const T*)c, len); break;
+            default: batch_inverse<F>(gpu, s, (T*)a, (const T*)b, len); break;
+            }
+            return rust_ok();
+        });
+    });
 }
 
 extern "C" RustError sppark_b200_prefix_op_dev(int field, int op, void* d_out, const void* d_inp, size_t len,
                                                void* stream)
 {
     if (op != 0 && op != 1) return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_prefix_op_dev: op is 0 (add) or 1 (multiply)");
-    return run_any(field, op == 0 ? WHAT_PREFIX_ADD : WHAT_PREFIX_MUL, d_out, d_inp, 0, nullptr, len, 0, stream);
+    return run(field, op == 0 ? WHAT_PREFIX_ADD : WHAT_PREFIX_MUL, d_out, d_inp, 0, nullptr, len, 0, stream);
 }
 
 extern "C" RustError sppark_b200_div_by_x_minus_z_dev(int field, void* d_inout, size_t len, const void* z,
                                                       int rotate, void* stream)
 {
     if (z == nullptr) return rust_err(-(int)cudaErrorInvalidValue, "sppark_b200_div_by_x_minus_z_dev: z is null");
-    return run_any(field, WHAT_DIV, d_inout, nullptr, 0, z, len, rotate != 0, stream);
+    return run(field, WHAT_DIV, d_inout, nullptr, 0, z, len, rotate != 0, stream);
 }
 
 extern "C" RustError sppark_b200_evaluate_dev(int field, void* d_ret, const void* d_x, size_t n,
                                               const void* d_coeffs, size_t len, void* stream)
-{   return run_any(field, WHAT_EVAL, d_ret, d_x, n, d_coeffs, len, 0, stream);   }
+{   return run(field, WHAT_EVAL, d_ret, d_x, n, d_coeffs, len, 0, stream);   }
 
 extern "C" RustError sppark_b200_batch_inverse_dev(int field, void* d_out, const void* d_inp, size_t len,
                                                    void* stream)
-{   return run_any(field, WHAT_INV, d_out, d_inp, 0, nullptr, len, 0, stream);   }
+{   return run(field, WHAT_INV, d_out, d_inp, 0, nullptr, len, 0, stream);   }

@@ -42,6 +42,29 @@ inline RustError rust_ok() { return RustError{0, nullptr}; }
 inline RustError rust_err(int code, const std::string& msg)
 {   return RustError{code, msg.empty() ? nullptr : strdup(msg.c_str())};   }
 
+// fn() for a C entry point: what it throws becomes the returned error instead of leaving the library
+template<class Fn> RustError guarded(Fn&& fn)
+{
+    try {
+        return fn();
+    } catch (const cuda_error& e) {
+        return rust_err(e.code(), e.what());
+    } catch (const std::exception& e) {
+        return rust_err(-1, e.what());
+    }
+}
+
+// raises kernel K's dynamic shared-memory limit to `bytes` once per device (function attributes
+// are per device context); static, as every translation unit has its own copy of a kernel
+template<auto K> static void smem_opt_in(int dev, int bytes)
+{
+    static bool done[64];
+    if (!done[dev & 63]) {
+        CUDA_OK(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        done[dev & 63] = true;
+    }
+}
+
 extern std::atomic<uint64_t> g_launch_count;      // defined in api.cu
 
 // Optional phase timing (bench.py's roofline leg): when enabled, the drivers drop CUDA events
