@@ -314,6 +314,25 @@ RustError sppark_b200_msm_ctx_invoke_batch(sppark_b200_msm_ctx *ctx, void *out_j
 RustError sppark_b200_msm_dev_batch(int curve, void *out_jacobians, const void *d_points, size_t npoints,
                                     const void *d_scalars, size_t batch, uint32_t scalar_bytes, uint32_t nbits,
                                     void *stream);
+/* Scalar multiplication of point arrays: out[i] = s_i * P_i for i < npoints, as packed affine {X, Y} rows
+ * (affine_bytes each, infinity = (0, 0)) -- the format sppark_b200_msm_ctx_create and mult_pippenger take.
+ * Scalars use the format of sppark_b200_msm_bits: scalar_bytes = 4, 8, 16 or 32, plain integers (not
+ * Montgomery form); bits from nbits up are ignored.  s_i is taken as an integer, not reduced mod r.
+ * One lane per point runs a signed 5-bit window ladder (DESIGN.md section 5e); it is not constant-time.
+ *   _dev: device memory, enqueued on `stream` without a synchronisation.  d_out == d_points (in place) is
+ *     allowed, any other overlap of the output with the inputs is refused; d_scalars aligned as for
+ *     sppark_b200_msm_dev_bits.
+ *   host entry: input rows as sppark_b200_msm reads them (ffi_affine_sz 0: packed rows; larger: rows with
+ *     an infinity flag after Y); the output is packed rows.  Synchronised before return.
+ * An unknown curve, a bad scalar format, a null pointer with npoints > 0, npoints >= 2^31, a partial
+ * overlap, misaligned device scalars or a bad host stride is refused with -cudaErrorInvalidValue before
+ * any device work, the output untouched.  npoints == 0 is a no-op. */
+RustError sppark_b200_scale_points_dev(int curve, void *d_out, const void *d_points, size_t npoints,
+                                       const void *d_scalars, uint32_t scalar_bytes, uint32_t nbits,
+                                       void *stream);
+RustError sppark_b200_scale_points(int curve, void *out_affine, const void *points_affine, size_t npoints,
+                                   const void *scalars, size_t ffi_affine_sz, uint32_t scalar_bytes,
+                                   uint32_t nbits);
 
 /* synthetic inputs: d_out[i] = (i+1)*G as packed affine points in DEVICE memory (the role of
  * util::generate_points_scalars, poc/msm-cuda/src/util.rs:11-38); enqueued on `stream`. */

@@ -57,7 +57,11 @@ _SIGS = {
                                          C.c_uint32],
     "sppark_b200_msm_dev_batch": [C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_uint32,
                                   C.c_uint32, C.c_void_p],
-    "sppark_b200_generate_points_dev": [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p],
+    "sppark_b200_scale_points_dev": [C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint32, C.c_uint32,
+                                     C.c_void_p],
+    "sppark_b200_scale_points": [C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_uint32,
+                                 C.c_uint32],
+    "sppark_b200_generate_points_dev":[C.c_int, C.c_void_p, C.c_size_t, C.c_void_p],
     "sppark_b200_msm_combine": [C.c_int, C.c_void_p, C.c_void_p, C.c_size_t],
     "sppark_b200_selftest_field": [C.c_int, C.c_int, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p],
     "sppark_b200_lde_powers_dev": [C.c_int, C.c_void_p, C.c_uint32, C.c_void_p],

@@ -24,6 +24,11 @@ struct curve_ops {
                                 uint32_t nbits);
     RustError (*dev_batch)(void* out, const void* d_points, size_t npoints, const void* d_scalars, size_t batch,
                            void* stream, uint32_t scalar_bytes, uint32_t nbits);
+    // out[i] = s_i * P_i as packed affine rows (msm_scale.cuh): host rows at `stride` bytes, or device rows
+    RustError (*scale)(void* out, const void* points, size_t npoints, const void* scalars, size_t stride,
+                       bool has_flag, uint32_t scalar_bytes, uint32_t nbits);
+    RustError (*scale_dev)(void* d_out, const void* d_points, size_t npoints, const void* d_scalars,
+                           uint32_t scalar_bytes, uint32_t nbits, void* stream);
     size_t affine_bytes, jacobian_bytes;        // packed {X, Y} and {X, Y, Z}
 };
 

@@ -315,6 +315,71 @@ extern "C" RustError sppark_b200_msm_dev_batch(int curve, void* out_jacobians, c
     return c->dev_batch(out_jacobians, d_points, npoints, d_scalars, batch, stream, scalar_bytes, nbits);
 }
 
+// ---- scalar multiplication of point arrays: out[i] = s_i * P_i, packed affine rows ---------------
+// Every refusal comes before any device work and leaves the output as it was.
+static bool overlaps(const void* a, size_t a_bytes, const void* b, size_t b_bytes)
+{
+    const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
+    return x < y + b_bytes && y < x + a_bytes;
+}
+
+// the checks both entries share; code 0 and *done = false when the call goes on
+static RustError check_scale(const char* entry, const curve_ops* c, void* out, const void* points, size_t npoints,
+                             const void* scalars, size_t stride, uint32_t scalar_bytes, uint32_t nbits, bool* done)
+{
+    *done = true;
+    const std::string e(entry);
+    if (c == nullptr) return rust_err(-(int)cudaErrorInvalidValue, e + ": unknown curve");
+    const RustError f = check_scalar_format(entry, c, nullptr, scalar_bytes, nbits);
+    if (f.code != 0) return f;
+    if (npoints == 0) return rust_ok();
+    if (out == nullptr || points == nullptr || scalars == nullptr)
+        return rust_err(-(int)cudaErrorInvalidValue, e + ": null pointer");
+    if (npoints >= (1ull << 31)) return rust_err(-(int)cudaErrorInvalidValue, e + ": npoints must be < 2^31");
+    const size_t out_bytes = npoints * c->affine_bytes;
+    if ((overlaps(out, out_bytes, points, npoints * stride) && !(out == points && stride == c->affine_bytes)) ||
+        overlaps(out, out_bytes, scalars, npoints * scalar_bytes))
+        return rust_err(-(int)cudaErrorInvalidValue, e + ": the output may be the points (in place) but may not "
+                                                         "overlap them or the scalars otherwise");
+    *done = false;
+    return rust_ok();
+}
+
+extern "C" RustError sppark_b200_scale_points_dev(int curve, void* d_out, const void* d_points, size_t npoints,
+                                                  const void* d_scalars, uint32_t scalar_bytes, uint32_t nbits,
+                                                  void* stream)
+{
+    const char* entry = "sppark_b200_scale_points_dev";
+    const curve_ops* c = curve_of(curve);
+    bool done;
+    const RustError e = check_scale(entry, c, d_out, d_points, npoints, d_scalars, c ? c->affine_bytes : 0,
+                                    scalar_bytes, nbits, &done);
+    if (e.code != 0 || done) return e;
+    if ((uintptr_t)d_scalars % (scalar_bytes < 16 ? scalar_bytes : 16) != 0)   // one aligned load per scalar
+        return rust_err(-(int)cudaErrorInvalidValue, std::string(entry) + ": d_scalars must be aligned to "
+                                                                          "min(scalar_bytes, 16) bytes");
+    return c->scale_dev(d_out, d_points, npoints, d_scalars, scalar_bytes, nbits, stream);
+}
+
+extern "C" RustError sppark_b200_scale_points(int curve, void* out_affine, const void* points_affine, size_t npoints,
+                                              const void* scalars, size_t ffi_affine_sz, uint32_t scalar_bytes,
+                                              uint32_t nbits)
+{
+    const char* entry = "sppark_b200_scale_points";
+    const curve_ops* c = curve_of(curve);
+    const size_t stride = c == nullptr ? 0 : ffi_affine_sz ? ffi_affine_sz : c->affine_bytes;
+    const bool has_flag = c != nullptr && ffi_affine_sz > c->affine_bytes;
+    bool done;
+    const RustError e = check_scale(entry, c, out_affine, points_affine, npoints, scalars, stride, scalar_bytes, nbits,
+                                    &done);
+    if (e.code != 0 || done) return e;
+    if (stride < c->affine_bytes + (has_flag ? 1 : 0))
+        return rust_err(-(int)cudaErrorInvalidValue, std::string(entry) + ": affine stride too small");
+    if (stride % 4 != 0)                         // rows are packed on the device with 32-bit loads
+        return rust_err(-(int)cudaErrorInvalidValue, std::string(entry) + ": affine stride must be a multiple of 4 bytes");
+    return c->scale(out_affine, points_affine, npoints, scalars, stride, has_flag, scalar_bytes, nbits);
+}
+
 extern "C" void sppark_b200_msm_ctx_free(sppark_b200_msm_ctx* ctx)
 {
     if (ctx == nullptr) return;

@@ -5,6 +5,7 @@
 #include "msm_core.cuh"
 #include "msm_pair.cuh"
 #include "msm_table.cuh"
+#include "msm_scale.cuh"
 
 namespace msm {
 
@@ -714,6 +715,58 @@ void build_table(uint32_t* d_table, size_t npoints, const Config& cfg, const str
         table_double_kernel<F><<<(n + 127) / 128, 128, 0, stream>>>(d_table, first, n, steps, cfg.copies, xyzz, zzz);
         pair_invert_kernel<F><<<((ns + PAIR_M - 1) / PAIR_M + 127) / 128, 128, 0, stream>>>(zzz, ns);
         table_normalize_kernel<F><<<(ns + 127) / 128, 128, 0, stream>>>(xyzz, zzz, npoints, first, n, ns, d_table);
+        COUNT_LAUNCH(); COUNT_LAUNCH(); COUNT_LAUNCH();
+        CUDA_OK(cudaGetLastError());
+    }
+}
+
+// ---- scalar multiplication of point arrays (msm_scale.cuh) --------------------------------------
+template<class F, uint32_t SW>
+__global__ void __launch_bounds__(128)
+scale_ladder_kernel(const uint32_t* points, const uint32_t* scalars, uint32_t nbits, uint32_t n, uint32_t* xyzz,
+                    uint32_t* zzz)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) scale_ladder_body<F, SW>(points, scalars, nbits, xyzz, zzz, i);
+}
+
+template<class F>
+__global__ void __launch_bounds__(128)
+scale_normalize_kernel(const uint32_t* xyzz, const uint32_t* zzz_inv, uint32_t n, uint32_t* out)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) normalize_to_row<F>(xyzz, zzz_inv, i, out + (size_t)i * 2 * F::N);
+}
+
+// points per chunk: SCALE_CHUNK, or SPPARK_B200_SCALE_CHUNK (tests: chunk boundaries at small sizes)
+inline size_t scale_chunk()
+{
+    const char* env = getenv("SPPARK_B200_SCALE_CHUNK");
+    const size_t v = env ? strtoull(env, nullptr, 10) : 0;
+    return v ? std::min(v, SCALE_CHUNK) : SCALE_CHUNK;
+}
+
+// d_out[i] = s_i * d_points[i], packed affine rows, enqueued on `stream`; d_out == d_points is allowed
+// (a chunk's points are read by its ladder before its normalise writes the same rows)
+template<class F>
+void scale_points(uint32_t* d_out, const uint32_t* d_points, size_t npoints, const uint32_t* d_scalars,
+                  uint32_t scalar_bytes, uint32_t nbits, const stream_t& stream)
+{
+    if (npoints == 0) return;
+    const size_t chunk = std::min(npoints, scale_chunk()), SW = scalar_bytes / 4;
+    dev_ptr_t<uint32_t> xyzz(chunk * 4 * F::N, stream), zzz(chunk * F::N, stream);
+    for (size_t first = 0; first < npoints; first += chunk) {
+        const uint32_t n = (uint32_t)std::min(chunk, npoints - first), blocks = (n + 127) / 128;
+        const uint32_t* p = d_points + first * 2 * F::N;
+        const uint32_t* s = d_scalars + first * SW;
+        switch (SW) {
+        case 1: scale_ladder_kernel<F, 1><<<blocks, 128, 0, stream>>>(p, s, nbits, n, xyzz, zzz); break;
+        case 2: scale_ladder_kernel<F, 2><<<blocks, 128, 0, stream>>>(p, s, nbits, n, xyzz, zzz); break;
+        case 4: scale_ladder_kernel<F, 4><<<blocks, 128, 0, stream>>>(p, s, nbits, n, xyzz, zzz); break;
+        default: scale_ladder_kernel<F, 8><<<blocks, 128, 0, stream>>>(p, s, nbits, n, xyzz, zzz); break;
+        }
+        pair_invert_kernel<F><<<((n + PAIR_M - 1) / PAIR_M + 127) / 128, 128, 0, stream>>>(zzz, n);
+        scale_normalize_kernel<F><<<blocks, 128, 0, stream>>>(xyzz, zzz, n, d_out + first * 2 * F::N);
         COUNT_LAUNCH(); COUNT_LAUNCH(); COUNT_LAUNCH();
         CUDA_OK(cudaGetLastError());
     }

@@ -314,6 +314,80 @@ RustError msm_dev(void* out, const void* d_points, size_t npoints, const void* d
                   uint32_t scalar_bytes, uint32_t nbits)
 {   return msm_dev_batch<F>(out, d_points, npoints, d_scalars, 1, stream, scalar_bytes, nbits);   }
 
+// ---- scalar multiplication of point arrays (msm_scale.cuh); the arguments are checked in msm.cu ----
+// device rows and scalars, enqueued on the caller's stream without a synchronisation
+template<class F>
+RustError scale_dev(void* d_out, const void* d_points, size_t npoints, const void* d_scalars, uint32_t scalar_bytes,
+                    uint32_t nbits, void* stream)
+{
+    try {
+        (void)gpu_of_current_device();          // the device's pool and stack settings; fails without a device
+        const stream_t s((cudaStream_t)stream);
+        msm::scale_points<F>((uint32_t*)d_out, (const uint32_t*)d_points, npoints, (const uint32_t*)d_scalars,
+                             scalar_bytes, nbits, s);
+    } catch (const cuda_error& e) {
+        return rust_err(e.code(), e.what());
+    } catch (const std::exception& e) {
+        return rust_err(-1, e.what());
+    }
+    return rust_ok();
+}
+
+// host rows (packed or flagged at `stride` bytes) -> host packed rows.  Per chunk, on one stream:
+// upload, the three steps in place on the uploaded rows, download.  The arithmetic outweighs the
+// transfers many times over, so they are not overlapped.
+template<class F>
+RustError scale_host(void* out, const void* points, size_t npoints, const void* scalars, size_t stride, bool has_flag,
+                     uint32_t scalar_bytes, uint32_t nbits)
+{
+    constexpr size_t PB = 2 * F::N * 4;
+    try {
+        const gpu_t& gpu = select_gpu(-1);
+        gpu.select();
+        const stream_t& s = gpu[0];
+        const bool packed = stride == PB && !has_flag;
+        const size_t chunk = std::min(npoints, msm::scale_chunk());
+        dev_ptr_t<uint32_t> d_pts(chunk * (PB / 4), s), d_sc(chunk * scalar_bytes / 4, s);
+        dev_ptr_t<uint8_t> d_raw(packed ? 1 : chunk * stride, s);
+        struct drain_t {
+            const stream_t& s;
+            bool armed = true;
+            ~drain_t() { if (armed) (void)cudaStreamSynchronize(s); }
+        } drain{s};
+        const bool pageable = stager_t::is_pageable(points) || stager_t::is_pageable(scalars) ||
+                              stager_t::is_pageable(out);
+        std::unique_lock<std::mutex> stage_lock(gpu.stage_mtx, std::defer_lock);
+        if (pageable) stage_lock.lock();
+        auto upload = [&](void* dst, const void* src, size_t bytes) {
+            if (pageable && stager_t::is_pageable(src)) gpu.stager().HtoD(s, dst, src, bytes);
+            else s.HtoD(dst, src, bytes);
+        };
+        for (size_t first = 0; first < npoints; first += chunk) {
+            const size_t n = std::min(chunk, npoints - first);
+            upload(d_sc, (const uint8_t*)scalars + first * scalar_bytes, n * scalar_bytes);
+            if (packed) {
+                upload(d_pts, (const uint8_t*)points + first * PB, n * PB);
+            } else {
+                upload(d_raw, (const uint8_t*)points + first * stride, n * stride);
+                uint32_t blocks = (uint32_t)std::min<size_t>((n + 255) / 256, (size_t)gpu.sm_count() * 8);
+                msm::pack_points_kernel<<<blocks, 256, 0, s>>>(d_raw, stride, PB / 4, has_flag, d_pts, (uint32_t)n);
+                COUNT_LAUNCH();
+                CUDA_OK(cudaGetLastError());
+            }
+            msm::scale_points<F>(d_pts, d_pts, n, d_sc, scalar_bytes, nbits, s);
+            uint8_t* dst = (uint8_t*)out + first * PB;
+            if (pageable && stager_t::is_pageable(out)) gpu.stager().DtoH(s, dst, d_pts, n * PB);
+            else s.DtoH(dst, d_pts, n * PB);
+        }
+        s.sync();
+        drain.armed = false;
+    } catch (const cuda_error& e) {
+        return rust_err(e.code(), e.what());
+    } catch (const std::exception& e) {
+        return rust_err(-1, e.what());
+    }
+    return rust_ok();
+}
 
 // ---- synthetic inputs: out[i] = (i+1)*G, affine (role of util::generate_points_scalars,
 // poc/msm-cuda/src/util.rs:11-38, which replicates 2^11 random points) ------------------------
@@ -394,7 +468,7 @@ constexpr curve_ops curve_row()
 {
     typedef typename G::F F;
     return {msm_host<F, Fr>, msm_dev<F>, gen_points<G>, combine<F>, msm_preload<F>, msm_resident<F, Fr>,
-            msm_resident_batch<F, Fr>, msm_dev_batch<F>, 2 * F::N * 4, 3 * F::N * 4};
+            msm_resident_batch<F, Fr>, msm_dev_batch<F>, scale_host<F>, scale_dev<F>, 2 * F::N * 4, 3 * F::N * 4};
 }
 
 }  // namespace

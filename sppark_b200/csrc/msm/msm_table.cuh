@@ -30,14 +30,13 @@ HD void table_double_body(const uint32_t* packed, size_t first, uint32_t n, uint
     }
 }
 
-// slot = (k-1) n + i of the chunk [first, first + n) -> packed affine row k * npoints + first + i
+// XYZZ point `slot` of the scratch and its inverted ZZZ -> packed affine row: u = 1/ZZZ,
+// x = X (ZZ u)^2, y = Y u; infinity -> (0, 0).  Shared by the table build and scale_points
+// (msm_scale.cuh).
 template<class F>
-HD void table_normalize_body(const uint32_t* xyzz, const uint32_t* zzz_inv, size_t npoints, size_t first,
-                             uint32_t n, uint32_t* table, uint32_t slot)
+HD void normalize_to_row(const uint32_t* xyzz, const uint32_t* zzz_inv, uint32_t slot, uint32_t* row)
 {
-    const uint32_t k = slot / n + 1, i = slot - (k - 1) * n;
     const ec::xyzz_t<F> acc = load_bucket<F>(xyzz, slot);
-    uint32_t* row = table + ((size_t)k * npoints + first + i) * 2 * F::N;
     if (acc.is_inf()) {
         pair_store_f<F>(row, F::zero());
         pair_store_f<F>(row + F::N, F::zero());
@@ -47,6 +46,15 @@ HD void table_normalize_body(const uint32_t* xyzz, const uint32_t* zzz_inv, size
     const F t = acc.ZZ * u;                             // 1 / Z
     pair_store_f<F>(row, acc.X * t.sqr());
     pair_store_f<F>(row + F::N, acc.Y * u);
+}
+
+// slot = (k-1) n + i of the chunk [first, first + n) -> packed affine row k * npoints + first + i
+template<class F>
+HD void table_normalize_body(const uint32_t* xyzz, const uint32_t* zzz_inv, size_t npoints, size_t first,
+                             uint32_t n, uint32_t* table, uint32_t slot)
+{
+    const uint32_t k = slot / n + 1, i = slot - (k - 1) * n;
+    normalize_to_row<F>(xyzz, zzz_inv, slot, table + ((size_t)k * npoints + first + i) * 2 * F::N);
 }
 
 }  // namespace msm

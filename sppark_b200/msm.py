@@ -251,6 +251,53 @@ def msm_dev_batch(curve, d_points, d_scalars, nbits=None, stream=None):
     return out
 
 
+def scale_points(curve, points, scalars, nbits=None):
+    """out[i] = scalars[i] * points[i] on the GPU, host arrays: points packed affine (n, 2*limbs) uint64 or
+    rows with an infinity-flag word appended (n, 2*limbs + 1); scalars as for msm() ((n, 4) or (n, 2)
+    uint64, (n,) uint64 or uint32; plain integers, not reduced mod r, bits from `nbits` up ignored).
+    Returns (n, 2*limbs) uint64 packed affine rows, infinity (0, 0) -- rows MsmContext and msm() take as
+    they are.  Not constant-time (DESIGN.md section 5e)."""
+    fmt = _host_format(scalars, False, nbits) or (32, 255)
+    _check_compact(points, scalars)
+    nl = _LIMBS[curve]
+    assert points.ndim == 2 and points.shape[1] in (2 * nl, 2 * nl + 1)
+    out = np.zeros((points.shape[0], 2 * nl), dtype=np.uint64)
+    ffi = 0 if points.shape[1] == 2 * nl else points.strides[0]
+    err = _lib.lib().sppark_b200_scale_points(curve, out.ctypes.data, points.ctypes.data, points.shape[0],
+                                              scalars.ctypes.data, ffi, *fmt)
+    _lib.check(err)
+    return out
+
+
+def scale_points_dev(curve, d_points, d_scalars, nbits=None, out=None, stream=None):
+    """out[i] = d_scalars[i] * d_points[i] with torch CUDA tensors: d_points packed affine (n, 2*limbs)
+    int64, d_scalars as for msm_dev ((n, 4) or (n, 2) int64, (n,) int64 or int32).  `out` (a tensor of
+    d_points' shape, or d_points itself for in place) or a new tensor receives the packed affine rows.
+    The work is enqueued on `stream` (default: the current stream) and not waited for."""
+    import torch
+    nl = _LIMBS[curve]
+    assert d_points.is_cuda and d_scalars.is_cuda and d_points.is_contiguous() and d_scalars.is_contiguous()
+    if d_points.ndim != 2 or d_points.shape[1] != 2 * nl:
+        raise ValueError(f"d_points must be (n, {2 * nl}) packed affine rows")
+    sbytes = _scalar_bytes(d_scalars, torch.int64, torch.int32)
+    if sbytes is None:
+        raise TypeError("scalars must be (n, 4) or (n, 2) int64, (n,) int64 or (n,) int32")
+    fmt = _scalar_format(sbytes, False, nbits) or (32, 255)
+    n = d_points.shape[0]
+    if d_scalars.shape[0] != n:
+        raise ValueError("length mismatch")
+    if out is None:
+        out = torch.empty_like(d_points)
+    elif out.shape != d_points.shape or out.device != d_points.device or not out.is_contiguous():
+        raise ValueError("out must be a contiguous tensor of d_points' shape on its device")
+    with torch.cuda.device(d_points.device):
+        s = stream if stream is not None else torch.cuda.current_stream().cuda_stream
+        err = _lib.lib().sppark_b200_scale_points_dev(curve, out.data_ptr(), d_points.data_ptr(), n,
+                                                      d_scalars.data_ptr(), fmt[0], fmt[1], s)
+    _lib.check(err)
+    return out
+
+
 def generate_points_dev(curve, n, device=None):
     """(n, 2*limbs) int64 CUDA tensor holding (i+1)*G, i < n, as packed Montgomery affine points."""
     import torch
