@@ -240,7 +240,14 @@ RustError sppark_b200_peer_open(const void *ipc_handle_64, void **d_ptr);
 RustError sppark_b200_peer_close(void *d_ptr);
 RustError sppark_b200_peer_free(void *d_ptr);
 
-/* MSM on any supported curve with host pointers (mult_pippenger's signature + curve id;
+/* Output on failure, for every entry that returns Jacobian points (mult_pippenger*, the MSM entries
+ * below and sppark_b200_msm_combine): once the size of the output is known -- the curve id is valid (for
+ * the _ctx_invoke entries: the context is not null) and batch * jacobian_bytes fits a size_t --, every
+ * failure sets all output points to infinity (all-zero), refusals of bad arguments included.  An unknown
+ * curve or a null context leaves the output as it was.  Bad arguments are refused with
+ * -cudaErrorInvalidValue.
+ *
+ * MSM on any supported curve with host pointers (mult_pippenger's signature + curve id;
  * the reference has no PoC boundary for Pasta, SURVEY.md section 8d config 4). */
 RustError sppark_b200_msm(int curve, void *out_jacobian, const void *points_affine,
                           size_t npoints, const void *scalars, size_t ffi_affine_sz);
@@ -254,7 +261,7 @@ RustError sppark_b200_msm_ex(int curve, void *out_jacobian, const void *points_a
  * 32-byte layout), scalar_bytes = 4, 8, 16 or 32; bits from nbits up are ignored, 1 <= nbits <=
  * min(255, 8 * scalar_bytes).  Plain integers, no Montgomery flag.  The MSM runs ceil((nbits + 1) / c)
  * windows instead of ceil(256 / c) and moves scalar_bytes per scalar; nbits = 255 with 32-byte scalars
- * is sppark_b200_msm_ex(..., 0).  A bad format returns -cudaErrorInvalidValue and infinity. */
+ * is sppark_b200_msm_ex(..., 0). */
 RustError sppark_b200_msm_bits(int curve, void *out_jacobian, const void *points_affine, size_t npoints,
                                const void *scalars, size_t ffi_affine_sz, uint32_t scalar_bytes, uint32_t nbits);
 /* One MSM sharded by point-chunk over GPUs of this process (SURVEY.md section 8e): chunk i of the points /
@@ -303,8 +310,7 @@ RustError sppark_b200_msm_dev_bits(int curve, void *out_jacobian, const void *d_
  * with vector b.  The vectors run in groups that share one sort, accumulate, reduce and finish.
  * batch == 0 is a no-op; npoints == 0 gives batch points at infinity.  A bad format, npoints past the
  * context's count, batch * npoints * scalar_bytes overflowing size_t or misaligned device scalars are
- * refused with -cudaErrorInvalidValue before any device work, every output set to infinity (not with
- * a null context or an unknown curve: the output size is then unknown, and nothing is written).
+ * refused before any device work.
  *   _ctx_invoke_batch: host scalars against the first npoints preloaded points of a plain or
  *     precomputed context; the scalars of the next group are uploaded while a group computes.
  *   _dev_batch: device points and scalars (aligned as for sppark_b200_msm_dev_bits); the work runs on

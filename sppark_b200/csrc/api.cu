@@ -106,7 +106,7 @@ static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
 
 extern "C" RustError sppark_b200_peer_alloc(size_t bytes, void** d_ptr, void* ipc_handle)
 {
-    try {
+    return guarded([&] {
         if (d_ptr == nullptr || ipc_handle == nullptr) throw cuda_error(-(int)cudaErrorInvalidValue, "peer_alloc: null argument");
         (void)gpu_of_current_device();
         CUDA_OK(cudaMalloc(d_ptr, bytes ? bytes : 1));
@@ -114,24 +114,20 @@ extern "C" RustError sppark_b200_peer_alloc(size_t bytes, void** d_ptr, void* ip
         cudaError_t e = cudaIpcGetMemHandle(&h, *d_ptr);
         if (e != cudaSuccess) { (void)cudaFree(*d_ptr); *d_ptr = nullptr; CUDA_OK(e); }
         memcpy(ipc_handle, &h, sizeof(h));
-    } catch (const cuda_error& e) {
-        return rust_err(e.code(), e.what());
-    }
-    return rust_ok();
+        return rust_ok();
+    });
 }
 
 extern "C" RustError sppark_b200_peer_open(const void* ipc_handle, void** d_ptr)
 {
-    try {
+    return guarded([&] {
         if (d_ptr == nullptr || ipc_handle == nullptr) throw cuda_error(-(int)cudaErrorInvalidValue, "peer_open: null argument");
         (void)gpu_of_current_device();
         cudaIpcMemHandle_t h;
         memcpy(&h, ipc_handle, sizeof(h));
         CUDA_OK(cudaIpcOpenMemHandle(d_ptr, h, cudaIpcMemLazyEnablePeerAccess));
-    } catch (const cuda_error& e) {
-        return rust_err(e.code(), e.what());
-    }
-    return rust_ok();
+        return rust_ok();
+    });
 }
 
 extern "C" RustError sppark_b200_peer_close(void* d_ptr)

@@ -37,39 +37,37 @@ __global__ void selftest_kernel(int op, size_t n, uint32_t* r, const uint32_t* a
 }
 
 template<class F>
-static RustError selftest(int op, size_t n, void* r, const void* a, const void* b)
+static void selftest(int op, size_t n, void* r, const void* a, const void* b)
 {
-    try {
-        const gpu_t& gpu = select_gpu(-1);
-        const stream_t& s = gpu[0];
-        const size_t bytes = n * F::N * 4, in_bytes = op == 7 ? 2 * bytes : bytes;
-        dev_ptr_t<uint32_t> da(in_bytes / 4, s), db(in_bytes / 4, s), dr(n * F::N, s);
-        s.HtoD(da, a, in_bytes);
-        s.HtoD(db, b, in_bytes);
-        selftest_kernel<F><<<(unsigned)((n + 127) / 128), 128, 0, s>>>(op, n, dr, da, db);
-        COUNT_LAUNCH();
-        CUDA_OK(cudaGetLastError());
-        s.DtoH(r, dr, bytes);
-        s.sync();
-    } catch (const cuda_error& e) {
-        return rust_err(e.code(), e.what());
-    }
-    return rust_ok();
+    const gpu_t& gpu = select_gpu(-1);
+    const stream_t& s = gpu[0];
+    const size_t bytes = n * F::N * 4, in_bytes = op == 7 ? 2 * bytes : bytes;
+    dev_ptr_t<uint32_t> da(in_bytes / 4, s), db(in_bytes / 4, s), dr(n * F::N, s);
+    s.HtoD(da, a, in_bytes);
+    s.HtoD(db, b, in_bytes);
+    selftest_kernel<F><<<(unsigned)((n + 127) / 128), 128, 0, s>>>(op, n, dr, da, db);
+    COUNT_LAUNCH();
+    CUDA_OK(cudaGetLastError());
+    s.DtoH(r, dr, bytes);
+    s.sync();
 }
 
 extern "C" RustError sppark_b200_selftest_field(int field, int op, size_t n, void* r, const void* a, const void* b)
 {
-    switch (field) {
-    case 0: return selftest<ff::bls12_381_fp_t>(op, n, r, a, b);
-    case 1: return selftest<ff::bls12_381_fr_t>(op, n, r, a, b);
-    case 2: return selftest<ff::pallas_fp_t>(op, n, r, a, b);
-    case 3: return selftest<ff::vesta_fp_t>(op, n, r, a, b);
-    case 4: return selftest<ff::bn254_fp_t>(op, n, r, a, b);
-    case 5: return selftest<ff::bn254_fr_t>(op, n, r, a, b);
-    case 6: return selftest<ff::bls12_377_fp_t>(op, n, r, a, b);
-    case 7: return selftest<ff::bls12_377_fr_t>(op, n, r, a, b);
-    default: return rust_err(-(int)cudaErrorInvalidValue, "selftest: unknown field");
-    }
+    return guarded([&] {
+        switch (field) {
+        case 0: selftest<ff::bls12_381_fp_t>(op, n, r, a, b); break;
+        case 1: selftest<ff::bls12_381_fr_t>(op, n, r, a, b); break;
+        case 2: selftest<ff::pallas_fp_t>(op, n, r, a, b); break;
+        case 3: selftest<ff::vesta_fp_t>(op, n, r, a, b); break;
+        case 4: selftest<ff::bn254_fp_t>(op, n, r, a, b); break;
+        case 5: selftest<ff::bn254_fr_t>(op, n, r, a, b); break;
+        case 6: selftest<ff::bls12_377_fp_t>(op, n, r, a, b); break;
+        case 7: selftest<ff::bls12_377_fr_t>(op, n, r, a, b); break;
+        default: throw cuda_error(-(int)cudaErrorInvalidValue, "selftest: unknown field");
+        }
+        return rust_ok();
+    });
 }
 
 // ---- device self-test hook: the MSM's bucket sort alone (tests/test_msm_sort.py) -------------------
@@ -82,9 +80,9 @@ extern "C" RustError sppark_b200_selftest_msm_sort(size_t n, uint32_t wbits, uin
                                                    uint32_t* info)
 {
     using namespace msm;
-    if (n == 0 || n >= (1ull << 31) || wbits < 3 || wbits > 24 || cap > SORT_CAP)
-        return rust_err(-(int)cudaErrorInvalidValue, "selftest_msm_sort: bad arguments");
-    try {
+    return guarded([&] {
+        if (n == 0 || n >= (1ull << 31) || wbits < 3 || wbits > 24 || cap > SORT_CAP)
+            throw cuda_error(-(int)cudaErrorInvalidValue, "selftest_msm_sort: bad arguments");
         const gpu_t& gpu = select_gpu(-1);
         const stream_t& s = gpu[0];
         Config cfg = make_config(n);
@@ -113,8 +111,6 @@ extern "C" RustError sppark_b200_selftest_msm_sort(size_t n, uint32_t wbits, uin
         s.sync();
         for (uint32_t h = 0; h < ctrl[1]; h++) static_cast<uint32_t*>(heavy_slots)[h] = hl[3 * h];
         info[0] = cfg.nwins; info[1] = cfg.heavy; info[2] = ctrl[1]; info[3] = sort_lg_bins(cfg, n); info[4] = ctrl[3];
-    } catch (const cuda_error& e) {
-        return rust_err(e.code(), e.what());
-    }
-    return rust_ok();
+        return rust_ok();
+    });
 }

@@ -111,6 +111,23 @@ public:
     void sync() const { CUDA_OK(cudaStreamSynchronize(s)); }
 };
 
+// On a failure, waits for the work of one or two streams while the buffers it uses are still alive
+// (their stream-ordered frees run during unwinding); disarmed once the call has synchronised.
+class drain_t {
+    const stream_t &a, &b;
+public:
+    bool armed = true;
+    explicit drain_t(const stream_t& s) : a(s), b(s) {}
+    drain_t(const stream_t& s, const stream_t& t) : a(s), b(t) {}
+    drain_t(const drain_t&) = delete;
+    ~drain_t()
+    {
+        if (!armed) return;
+        (void)cudaStreamSynchronize(a);
+        if (&b != &a) (void)cudaStreamSynchronize(b);
+    }
+};
+
 // cudaEvent_t with a lifetime (no timing): destroyed on every exit path
 class event_t {
     cudaEvent_t e;
